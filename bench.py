@@ -1,15 +1,18 @@
 #!/usr/bin/env python
 """Headline benchmark (BASELINE.json): ResNet-50 training images/sec, bf16, 224x224 synthetic images, per-GPU batch
-256 (reference P1/03:81), N = 1/2/4/8 B200 (weak scaling), device-timed, max over ranks.
+256 (reference P1/03:81), N = 1/2/4/8 H100 (weak scaling), device-timed, max over ranks.
 
     python bench.py [--gpus N --steps K --warmup W]            # our engine (N>1: launched by torchrun)
     python bench.py --impl reference ...                        # the unmodified reference (not installable offline)
     python bench.py --impl torch-baseline ...                   # operative baseline: torch + cuDNN + NCCL (BASELINE.md §2)
+    python bench.py ... --dump-outputs DIR                      # also write the last timed step's outputs as .npy
 
 Prints ONE JSON line on rank 0.  `value` = kernel-only device time of K full training steps (forward, backward,
 fused all-reduce, optimizer) with the step captured in a CUDA graph and the input batch resident on the device;
 `e2e` = the same metric through the public API (`Trainer.fit` over the pinned ring loader): every step includes the
 host->device copy of its input batch from pinned memory and a device->host read of the step's loss/accuracy.
+Inputs and weights are seeded, so two builds run with the same arguments can be compared output for output
+(`--dump-outputs`).
 """
 from __future__ import annotations
 
@@ -28,7 +31,7 @@ METRIC = "resnet50_train_images_per_sec"
 
 
 class ClockSampler:
-    """Samples SM clocks / throttle reasons with nvidia-smi DURING the timed region (B200_PROFILING.md recipe)."""
+    """Samples SM clocks / throttle reasons with nvidia-smi DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -87,6 +90,24 @@ class ClockSampler:
                 "samples": len(sm), "power_w_max": max(power), "sm_mhz_min": sm_sorted[0]}
 
 
+DUMP_PARAM_SAMPLE = 1 << 20  # fp32 weights sampled for --dump-outputs (the full 25.6 M would be ~100 MB)
+
+
+def dump_outputs(out_dir: str, engine, loss: float, acc: float) -> None:
+    """What the timed training step returned in its last step, as float32 / float64 .npy files (~5 MB in all):
+    the loss and accuracy, the fp32 logits of the batch, and a fixed seeded sample of the updated fp32 weights."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float64))
+    np.save(os.path.join(out_dir, "accuracy.npy"), np.array([acc], dtype=np.float64))
+    np.save(os.path.join(out_dir, "logits.npy"), engine.logits.float().cpu().numpy())
+    n = engine.params.numel()
+    idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:min(n, DUMP_PARAM_SAMPLE)].sort().values
+    np.save(os.path.join(out_dir, "params_sample.npy"), engine.params.detach().cpu()[idx].numpy())
+
+
 def run_reference(args):
     # The reference tree holds Databricks notebooks only: no setup.py / pyproject, and its imports (tensorflow,
     # horovod, petastorm, pyspark, mlflow, hyperopt) are absent from the image and the offline wheelhouse.
@@ -114,8 +135,7 @@ def run_baseline_child(args, rank: int, world: int):
     base_port = int(os.environ.get("MASTER_PORT", "29500"))
     result, notes = None, []
     # N = 1: CUDA graph first, eager as the fallback.  N > 1: eager only - capturing the hook-launched NCCL all-reduces of
-    # the baseline in a CUDA graph did not complete on the 4-GPU box (child timed out at 150 s, profiles/r2_bench_w4.json);
-    # eager costs the baseline ~4 % at N = 1 (4,710 vs 4,891 img/s in round 1), it is what DDP users run.
+    # the baseline in a CUDA graph did not complete on a 4-GPU box; eager is what DDP users run.
     for attempt, graph in enumerate((True, False) if world == 1 else (False,)):
         env["MASTER_PORT"] = str(base_port + 23 + attempt)
         cmd = [sys.executable, script, "--steps", str(args.steps), "--warmup", str(args.warmup), "--batch",
@@ -204,6 +224,8 @@ def main():
     ap.add_argument("--baseline-timeout", type=int, default=200)
     ap.add_argument("--no-block-grad", action="store_true", help="A/B: block-gradient merge as separate reduce passes")
     ap.add_argument("--stem-bwd-fuse", action="store_true", help="A/B (opt-in): max-pool backward fused with the stem-BN backward")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's loss, accuracy, logits and a weight sample as .npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -272,6 +294,8 @@ def main():
     ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
     ms = float(dist.allreduce(ms, average=False).item()) if world == 1 else float(_max_over_ranks(ms))
     loss, acc = step.result()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, engine, loss, acc)
     # outside the timed region: after K data-parallel steps every rank must hold bit-identical fp32 master weights
     # (a gradient that was all-reduced before its producer finished would show up here)
     from b200ddl.utils import checksum_across_ranks
@@ -344,7 +368,7 @@ def main():
                        "optimizer": args.optimizer, "allreduce": algo_used,
                        "fused_allreduce_sgd": fused_used,
                        "cuda_graph": not args.no_graph, "overlap_wgrad": not args.no_overlap_wgrad, **cfg_flags,
-                       "l2": "activations per step are several GB (>> 126 MB L2); no explicit flush needed"},
+                       "l2": "activations per step are several GB (>> 50 MB L2); no explicit flush needed"},
             "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches_per_step * args.steps),
             "launches_per_step": int(launches_per_step), "loss": loss, "accuracy": acc,
             "params_identical_across_ranks": params_identical,

@@ -1,11 +1,11 @@
-"""Kernel-by-kernel numerics + timing checks on a real B200 (run through gpurun).
+"""Kernel-by-kernel numerics + timing checks on a real H100.
 
     python benchmarks/gpu_check.py <case> [<case> ...]
 
-Every case compares a hand-written sm_100a kernel against a plain PyTorch fp32 reference of the same op and
+Every case compares a hand-written sm_90a kernel against a plain PyTorch fp32 reference of the same op and
 prints one ``CHECK <name> ... PASS|FAIL`` line; timing cases print ``TIME`` lines (CUDA events, warm-up, median).
-The shell driver (benchmarks/run_gpu_checks.sh) runs each case in its own process under ``timeout`` so that a
-hung kernel cannot take the whole GPU call down.
+Run each case in its own process under ``timeout`` when checking a new kernel, so that one hung kernel cannot take the
+whole run down.
 """
 from __future__ import annotations
 
@@ -711,7 +711,7 @@ def case_block_grad():
 
 
 def case_head():
-    """Classifier head: FC forward / dgrad / wgrad on the tcgen05 GEMMs + softmax_ce_head + fc_bias_grad vs torch fp32."""
+    """Classifier head: FC forward / dgrad / wgrad on the wgmma GEMMs + softmax_ce_head + fc_bias_grad vs torch fp32."""
     ok = True
     e = ops.ext("_b200_ops")
     for N, K in ((256, 1000), (8, 5), (32, 10), (64, 200)):
@@ -941,7 +941,7 @@ def case_fused_infer():
 
 def case_mobilenet():
     """The reference's own model on native kernels: depthwise / stem kernels vs torch, then the whole frozen-base
-    MobileNetV2 engine (tcgen05 pointwise convs with folded-BN epilogues) vs the torch.nn module with the same weights."""
+    MobileNetV2 engine (wgmma pointwise convs with folded-BN epilogues) vs the torch.nn module with the same weights."""
     ok = True
     e = ops.ext("_b200_ops")
     g = torch.Generator(device=DEV).manual_seed(51)
@@ -1128,38 +1128,6 @@ def case_tails():
     return ok
 
 
-def case_umma_probe():
-    """Row-shifted SWIZZLE_128B descriptors: which (shift, base_offset) combinations read the right rows?"""
-    ext = ops.ext("_b200_probe")
-    g = torch.Generator(device=DEV).manual_seed(21)
-    T = torch.randn(160, 64, device=DEV, generator=g).to(torch.bfloat16)
-    B = torch.randn(64, 64, device=DEV, generator=g).to(torch.bfloat16)
-    ok0 = True
-    for shift in (0, 1, 2, 3, 7, 8, 9, 30):
-        ref = T[shift:shift + 128].float() @ B.float().t()
-        res = []
-        for bo in (False, True):
-            out = ext.umma_probe(T, B, shift, bo)
-            torch.cuda.synchronize()
-            res.append(rel_err(out, ref))
-        print(f"PROBE shift={shift:2d} err(base_offset=0)={res[0]:.3e} err(base_offset=(addr>>7)&7)={res[1]:.3e}", flush=True)
-        if shift == 0:
-            ok0 &= res[0] < 1e-2
-    # second question: 8-row groups at a stride other than 1024 bytes (2-D halo tiles need 1280 = a 10-pixel-wide row)
-    T2 = torch.randn(256, 64, device=DEV, generator=g).to(torch.bfloat16)
-    for sbo in (1024, 1152, 1280, 1536, 2048):
-        step = sbo // 128
-        for shift in (0, 1, 11, 22):
-            if shift + 15 * step + 8 > 256:
-                continue
-            rows = torch.cat([torch.arange(shift + gi * step, shift + gi * step + 8, device=DEV) for gi in range(16)])
-            ref = T2[rows].float() @ B.float().t()
-            out = ext.umma_probe(T2, B, shift, False, sbo)
-            torch.cuda.synchronize()
-            print(f"PROBE group_stride={sbo:5d} B ({step:2d} rows) shift={shift:2d} err={rel_err(out, ref):.3e}", flush=True)
-    return ok0
-
-
 def case_tma_probe():
     """TMA load pipeline alone (no MMA, no epilogue): time per box load for the shapes the 3x3 convs use or could use."""
     ext = ops.ext("_b200_probe")
@@ -1223,7 +1191,6 @@ CASES = {
     "mobilenet": case_mobilenet,
     "tails": case_tails,
     "engine_unfused_block_grad": lambda: case_engine(quick=True, fuse_block_grad=False),
-    "umma_probe": case_umma_probe,
 }
 
 if __name__ == "__main__":

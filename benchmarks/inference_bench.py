@@ -1,5 +1,5 @@
 """Batch-inference throughput (BASELINE.json config 4): the trained ResNet-50's forward (BN folded to running
-statistics, same tcgen05 conv kernels, CUDA graph) over synthetic images sharded across GPUs.
+statistics, same wgmma conv kernels, CUDA graph) over synthetic images sharded across GPUs.
 
     python benchmarks/inference_bench.py --images 100000                       # one GPU
     torchrun --nproc-per-node 8 ... benchmarks/inference_bench.py --images 1000000

@@ -1,6 +1,6 @@
 """Tiny launcher for ncu: runs ONE kernel family on one ResNet-50 layer shape a few times.
 
-    ncu --set full --clock-control none --import-source on -k regex:<kernel> -s 3 -c 1 -o gpurun_out/<name> \
+    ncu --set full --clock-control none --import-source on -k regex:<kernel> -s 3 -c 1 -o <name> \
         python benchmarks/ncu_target.py <what> <shape-name>
 
 what: fwd | fwd_stats | fwd_infer | dgrad | wgrad | bn_reduce | bn_apply | bn_bwd_apply | block_grad | stem_bwd_reduce | stem_bwd_apply | dwconv

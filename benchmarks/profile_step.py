@@ -1,5 +1,6 @@
 """Per-kernel time breakdown of one eager ResNet-50 training step (torch.profiler / CUPTI), written to
-gpurun_out/step_profile.txt.  Used to decide what to optimise next; the judged evidence is the ncu output."""
+profiles/step_profile.txt and profiles/step_kernels.txt (generated output, not tracked).  Used to decide what to
+optimise next."""
 import os
 import sys
 
@@ -25,15 +26,16 @@ with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
         step.run()
     torch.cuda.synchronize()
 tab = prof.key_averages().table(sort_by="cuda_time_total", row_limit=45, max_name_column_width=90)
-os.makedirs("gpurun_out", exist_ok=True)
-with open("gpurun_out/step_profile.txt", "w") as f:
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles")
+os.makedirs(OUT, exist_ok=True)
+with open(os.path.join(OUT, "step_profile.txt"), "w") as f:
     f.write(tab)
 # compact per-kernel summary (3 steps)
 rows = [(e.key, e.device_time_total / 3.0, e.count // 3) for e in prof.key_averages() if e.device_time_total > 0 and e.device_type.name == "CUDA"]
 rows.sort(key=lambda r: -r[1])
 tot = sum(r[1] for r in rows)
-with open("gpurun_out/step_kernels.txt", "w") as f:
+with open(os.path.join(OUT, "step_kernels.txt"), "w") as f:
     f.write(f"total device kernel time per step: {tot/1e3:.2f} ms\n")
     for k, t, c in rows[:60]:
         f.write(f"{t/1e3:9.3f} ms  {100*t/tot:5.1f}%  x{c:<4d} {k[:150]}\n")
-print(open("gpurun_out/step_kernels.txt").read())
+print(open(os.path.join(OUT, "step_kernels.txt")).read())

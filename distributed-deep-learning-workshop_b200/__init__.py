@@ -1,9 +1,9 @@
-"""b200ddl - a Blackwell (B200, sm_100a) native distributed deep-learning stack.
+"""b200ddl - a Hopper (H100, sm_90a) native distributed deep-learning stack.
 
 Capabilities mirror the notebook workflow of ``smellslikeml/distributed-deep-learning-workshop``
 (see SURVEY.md): table ETL -> sharded loader -> Keras-like trainer -> Horovod-like distributed runtime ->
 Hyperopt-like search -> MLflow-like tracking / registry / pyfunc -> batch inference, with the hot paths
-(conv/BN/ReLU stack, optimizers, gradient all-reduce, input pipeline) written as sm_100a CUDA/C++.
+(conv/BN/ReLU stack, optimizers, gradient all-reduce, input pipeline) written as sm_90a CUDA/C++.
 
 Sub-packages are imported lazily so that ``import b200ddl`` stays cheap:
 

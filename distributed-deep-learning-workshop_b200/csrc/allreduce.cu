@@ -1,4 +1,4 @@
-// Fused gradient all-reduce kernels for 2-8 B200s on one NVSwitch domain (SURVEY.md K1-K3, §5.8).
+// Fused gradient all-reduce kernels for 2-8 H100s on one NVSwitch domain (SURVEY.md K1-K3, §5.8).
 //
 // The reference reaches NCCL through Horovod's DistributedOptimizer and then runs separate scale / cast kernels.
 // Here ONE kernel does barrier -> reduce -> x(1/N) -> cast -> write-back -> barrier, reading and writing peer

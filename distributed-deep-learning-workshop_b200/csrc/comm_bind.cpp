@@ -68,7 +68,7 @@ struct Comm {
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   namespace py = pybind11;
-  m.doc() = "b200ddl fused all-reduce kernels over NVLink symmetric memory (sm_100a)";
+  m.doc() = "b200ddl fused all-reduce kernels over NVLink symmetric memory (sm_90a)";
   py::class_<Comm>(m, "Comm")
       .def(py::init<int64_t, int64_t, int64_t, int64_t, int64_t>(), py::arg("peer_bufs_dev"),
            py::arg("peer_flags_dev"), py::arg("mc_ptr"), py::arg("rank"), py::arg("world"))

@@ -53,7 +53,5 @@ struct TmaProbeParams {
 };
 // TMA load-throughput probe (csrc/tma_probe.cu): box loads into a ring of stages, consumer only releases them.
 void tma_probe_launch(const CUtensorMap& tm, const TmaProbeParams& p, int grid, cudaStream_t s);
-void umma_probe_launch(const CUtensorMap& tmT, const CUtensorMap& tmB, float* out, int shift, int use_base_offset,
-                       int t_rows, int sbo_bytes, cudaStream_t s);
 
 }  // namespace b200

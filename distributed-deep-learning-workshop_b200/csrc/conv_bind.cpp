@@ -1,4 +1,4 @@
-// pybind layer for the tcgen05 convolution kernels: validates tensors, derives the tiling, encodes the TMA
+// pybind layer for the wgmma convolution kernels: validates tensors, derives the tiling, encodes the TMA
 // descriptors once, and exposes launchable plan objects (static buffers => plans are reused under CUDA graphs).
 #include <ATen/cuda/CUDAContext.h>
 #include <torch/extension.h>
@@ -68,7 +68,7 @@ struct ConvPlan {
                 "weight must be bf16 [taps*Cout, Cin]");
     ConvParams& p = raw.p;
     std::memset(&p, 0, sizeof(p));
-    raw.block_n = cout % 256 == 0 ? 256 : (cout % 128 == 0 ? 128 : 64);
+    raw.block_n = cout % 128 == 0 ? 128 : 64;
     p.taps = taps;
     p.kblocks = (int)(cin / 64);
     p.cout = (int)cout;
@@ -111,11 +111,10 @@ struct ConvPlan {
       }
       raw.tmD = map_nhwc(out, 64, (int)bw, (int)bh, (int)bn);
     }
-    // Tile width: the widest N tile re-reads the A operand least, but a persistent grid of one CTA per SM pays for whole
-    // waves - e.g. 3x3 512->512 @7^2 at batch 256 is 98 M-tiles x 2 N-blocks = 196 tiles of 128x256 on 148 SMs = 2 waves at
-    // 66 % fill (ncu: tensor pipe 80 % busy, 59 us vs cuDNN 47), while 392 tiles of 128x128 fill 3 waves at 88 %.  The cost
-    // model is waves x tile width (the MMA time of a tile is proportional to its width); a narrower tile is taken only when
-    // it wins by >= 10 %.  B200DDL_BLOCK_N=256|128|64 forces a width (A/B measurements).
+    // Tile width: the wider N tile re-reads the A operand less, but a persistent grid of one CTA per SM pays for whole
+    // waves.  The cost model is waves x tile width (the MMA time of a tile is proportional to its width); the narrower
+    // tile is taken only when it wins by >= 10 %.  128 is the widest: the two consumer warpgroups hold a 64 x BLOCK_N fp32
+    // accumulator each in registers.  B200DDL_BLOCK_N=128|64 forces a width (A/B measurements).
     {
       const int cap_ = max_ctas > 0 ? (int)max_ctas : sm_count();
       auto cost = [&](int bn) {
@@ -127,7 +126,7 @@ struct ConvPlan {
         if (cout % bn == 0 && cost(bn) * 10 <= cost(best) * 9) best = bn;
       if (const char* f = std::getenv("B200DDL_BLOCK_N")) {
         const int v = std::atoi(f);
-        if ((v == 256 || v == 128 || v == 64) && cout % v == 0) best = v;
+        if ((v == 128 || v == 64) && cout % v == 0) best = v;
       }
       raw.block_n = best;
     }
@@ -144,16 +143,14 @@ struct ConvPlan {
                    raw.stats != 3) ? 1 : 0;
     }
     // Halo mode: a 3x3 stride-1 conv (9 taps on ONE view forming the full {-1,0,1}^2 offset grid, in any order) over
-    // full-width single-image boxes: one [bw x (bh+2)] load per horizontal offset serves its three vertical taps.
+    // full-width single-image boxes: one [bw x (bh+2)] load per horizontal offset serves its three vertical taps, read at
+    // row offsets 0 / bw / 2*bw - whole 1024 B swizzle atoms only when bw % 8 == 0.
     // B200DDL_NO_HALO=1 switches it off (A/B measurements).
     raw.halo = 0;
     {
       const char* off = std::getenv("B200DDL_NO_HALO");
-      // two-dimensional variant: 8-pixel-wide boxes, ONE [(bw+2) x (bh+2)] load per tile (B200DDL_HALO2D=1 opts in)
-      const char* h2 = std::getenv("B200DDL_HALO2D");
-      const bool two_d = (h2 && h2[0] == '1') && bw == 8 && bh <= 16 && (bw + 2) * (bh + 2) <= 224 && Wo % 8 == 0;
       bool ok = raw.res_b && p.mode == 1 && taps == 9 && views.size() == 1 && bn == 1 && !(off && off[0] == '1') &&
-                (two_d || (bw == views[0].size(2) && bw == Wo && bw * (bh + 2) <= 224));
+                bw % 8 == 0 && bw == views[0].size(2) && bw == Wo && bw * (bh + 2) <= 224;
       int8_t table[9];
       for (int i = 0; i < 9; ++i) table[i] = -1;
       for (int t = 0; ok && t < 9; ++t) {
@@ -161,12 +158,7 @@ struct ConvPlan {
         if (p.tap_map[t] != 0 || dwv < -1 || dwv > 1 || dhv < -1 || dhv > 1 || table[(dwv + 1) * 3 + (dhv + 1)] != -1) ok = false;
         else table[(dwv + 1) * 3 + (dhv + 1)] = (int8_t)t;
       }
-      if (ok && two_d) {
-        raw.halo = 2;
-        p.halo = 2;
-        p.halo_bytes = (int)((bw + 2) * (bh + 2) * 128);
-        raw.tmA[1] = map_nhwc(views[0], 64, (int)bw + 2, (int)bh + 2, 1);
-      } else if (ok) {
+      if (ok) {
         raw.halo = 1;
         p.halo = 1;
         p.halo_bytes = (int)(bw * (bh + 2) * 128);
@@ -341,6 +333,7 @@ struct WgradPlan {
     TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.is_contiguous() && dw.numel() == taps * cout * cin,
                 "dw must be fp32 [taps*Cout, Cin]");
     TORCH_CHECK(S >= 1 && S <= 4, "filter width 1..4");
+    // the unit's 64 x (64 * G) fp32 accumulator lives in the registers of one warpgroup: G <= 4 (N <= 256)
     WgradParams& p = raw.p;
     std::memset(&p, 0, sizeof(p));
     p.cout = (int)cout;
@@ -352,10 +345,8 @@ struct WgradPlan {
     if (S == 1) {
       p.cb_per_group = cin_blocks < 4 ? cin_blocks : 4;
       while (cin_blocks % p.cb_per_group) --p.cb_per_group;
-      p.acc_chunks = p.cb_per_group;
     } else {
-      p.cb_per_group = (cin_blocks >= 2 && S * 2 <= 6) ? 2 : 1;
-      p.acc_chunks = (int)S;
+      p.cb_per_group = (cin_blocks >= 2 && S * 2 <= 4) ? 2 : 1;
     }
     p.G = (int)S * p.cb_per_group;
     p.cgroups = cin_blocks / p.cb_per_group;
@@ -399,7 +390,7 @@ struct WgradPlan {
     const int stage_bytes = (p.a_chunks + p.G) * p.P * 128;
     // smem_budget < 227 KB leaves room for bandwidth-bound kernels to co-reside when wgrad runs on a side stream
     const int budget = (smem_budget > 0 && smem_budget < 232448) ? (int)smem_budget : 232448;
-    p.stages = (budget - 256) / stage_bytes;
+    p.stages = (budget - 256 - 1024) / stage_bytes;   // + barriers, + 1 KB to align the dynamic smem base
     if (p.stages > 8) p.stages = 8;
     TORCH_CHECK(p.stages >= 2, "wgrad stage does not fit shared memory");
     const int combos = p.co_blocks * p.groups;
@@ -491,7 +482,7 @@ struct StemPlan {
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   namespace py = pybind11;
-  m.doc() = "b200ddl tcgen05/TMA implicit-GEMM convolution kernels (sm_100a)";
+  m.doc() = "b200ddl wgmma/TMA implicit-GEMM convolution kernels (sm_90a)";
   py::class_<b200::ConvPlan>(m, "ConvPlan")
       .def(py::init<std::vector<at::Tensor>, at::Tensor, at::Tensor, std::vector<int64_t>, std::vector<int64_t>,
                     std::vector<int64_t>, int64_t, int64_t, int64_t, c10::optional<at::Tensor>,

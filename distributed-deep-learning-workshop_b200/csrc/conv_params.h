@@ -80,8 +80,7 @@ struct WgradParams {
   int mode;          // 0 = flat (2-D [M, C] maps), 1 = box (4-D NHWC maps)
   int P;             // pixels per k-iteration (multiple of 16, <= 128)
   int a_chunks;      // 64-channel chunks of dY per unit (1 if Cout == 64, else 2)
-  int G;             // 64-channel chunks of X per unit (1..6), ordered (ci-block, s)
-  int acc_chunks;    // chunks per accumulator: MMA N = 64 * acc_chunks
+  int G;             // 64-channel chunks of X per unit (1..4), ordered (ci-block, s): MMA N = 64 * G
   int S;             // filter width; a unit covers one filter row r (taps r*S .. r*S+S-1)
   int cb_per_group;  // ci 64-blocks per unit
   int cgroups;       // (Cin/64) / cb_per_group

@@ -1,13 +1,14 @@
-// Weight-gradient convolution kernel for sm_100a (tcgen05 + TMEM + TMA), split-K over pixels.
+// Weight-gradient convolution kernel for sm_90a (wgmma + TMA), split-K over pixels.
 //
 //   dW[tap][co][ci] += sum_px dY[px, co] * X_tap[px, ci]
 //
 // Both operands are "MN-major" for the tensor core (the reduction index, the pixel, is the slow smem dimension):
 // the very same TMA boxes the forward kernel loads ([P pixels] x [64 channels], SWIZZLE_128B) are consumed
-// directly with a_major = b_major = MN in the instruction descriptor, so there is no transpose pass.
-// A unit of work = (pixel chunk, 128-wide co block, group of <= 6 (tap, ci-block) chunks of one filter row);
-// the accumulators (up to 384 fp32 columns) live in TMEM for the whole pixel chunk and are flushed once with
-// 16-byte vector atomics (red.global.add.v4.f32) into the fp32 gradient buffer that the all-reduce consumes.
+// directly with the transpose flags of wgmma set, so there is no transpose pass.
+// A unit of work = (pixel chunk, 128-wide co block, group of G <= 4 (tap, ci-block) chunks of one filter row).
+// Warpgroup g (warps 4g .. 4g+3) owns co chunk g of the block; its 64 x (64 * G) fp32 accumulator lives in registers for
+// the whole pixel chunk and is flushed once with vector atomics into the fp32 gradient buffer that the all-reduce consumes.
+// Warp 8 is the TMA producer (lane j issues chunk j of a stage).
 #include <stdexcept>
 #include <string>
 
@@ -17,24 +18,31 @@
 namespace b200 {
 
 constexpr int kWgMaxStages = 8;
+constexpr int kWgConsumers = 256;
+constexpr int kWgThreads = kWgConsumers + 32;
 
-__global__ void __launch_bounds__(256, 1)
+template <int G>
+__device__ __forceinline__ void wgrad_mma(float (&acc)[32 * G], uint64_t da, uint64_t db) {
+  if constexpr (G == 1) wgmma_m64n64k16<1, 1>(acc, da, db);
+  else if constexpr (G == 2) wgmma_m64n128k16<1, 1>(acc, da, db);
+  else if constexpr (G == 3) wgmma_m64n192k16<1, 1>(acc, da, db);
+  else wgmma_m64n256k16<1, 1>(acc, da, db);
+}
+
+template <int G>
+__global__ void __launch_bounds__(kWgThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX0,
                   const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
                   const __grid_constant__ CUtensorMap tmX3, const __grid_constant__ WgradParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
+  uint8_t* smem = align_smem_1024(smem_raw);
   const int slot_bytes = p.P * 128;
-  const int stage_bytes = (p.a_chunks + p.G) * slot_bytes;
+  const int stage_bytes = (p.a_chunks + G) * slot_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
   uint64_t* full_bar = bars;                   // [stages]
   uint64_t* empty_bar = bars + kWgMaxStages;   // [stages]
-  uint64_t* tfull_bar = bars + 2 * kWgMaxStages;
-  uint64_t* tempty_bar = bars + 2 * kWgMaxStages + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kWgMaxStages + 2);
 
-  // provably warp-uniform (see conv_igemm.cuh): keeps the single-thread MMA loop free of per-instruction ELECT loops
+  // provably warp-uniform (see conv_igemm.cuh)
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
 
@@ -43,30 +51,18 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     tma_prefetch_desc(&tmX0);
     for (int i = 0; i < p.stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], kWgConsumers / 32);
     }
-    mbar_init(tfull_bar, 1);
-    mbar_init(tempty_bar, 4);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int combos = p.co_blocks * p.groups;
-  const int n_acc = p.G / p.acc_chunks;
-  const int acc_cols = 64 * p.acc_chunks;
 
-  if (warp == 0) {
+  if (warp == kWgConsumers / 32) {
     // ------------------------------------------------------------------ TMA producer (one warp; lane j issues chunk j)
     // All per-chunk parameters (tensor map, channel coordinate, tap offset) are hoisted out of the k loop and the
-    // <= 8 loads of a stage are issued by 8 lanes in parallel: a single thread doing the index arithmetic for every
-    // load was the bottleneck of this kernel (ncu: tensor pipe 26 % active, everything else idle).
-    const int n_loads = p.a_chunks + p.G;
+    // <= 6 loads of a stage are issued by 6 lanes in parallel.
+    const int n_loads = p.a_chunks + G;
     int stage = 0;
     uint32_t phase = 0;
     const uint32_t tx = static_cast<uint32_t>(stage_bytes);
@@ -129,114 +125,105 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      // ---------------------------------------------------------------- MMA issuer (one elected thread)
-      // elect.sync + integer barrier addresses: with `lane == 0` every tcgen05.mma / commit below was wrapped in an
-      // ELECT / PLOP3 / BRA.U.ANY serialisation loop (~10 extra instructions per MMA, 8-24 MMAs per stage).
-      const uint32_t idesc = umma_idesc_bf16(128, acc_cols, 1, 1);  // both operands MN-major
-      const uint32_t a_lbo = (p.a_chunks == 2) ? slot_bytes : 0;    // Cout == 64: rows 64..127 mirror rows 0..63
-      // descriptors differ only in the 14-bit start-address field: build one per stage up front, then add offsets
-      const uint64_t da0 = umma_desc_sw128(smem_u32(smem), a_lbo, 1024);
-      const uint64_t db0 = umma_desc_sw128(smem_u32(smem) + p.a_chunks * slot_bytes, slot_bytes, 1024);
-      const uint32_t stage_step = static_cast<uint32_t>(stage_bytes) >> 4;
-      const uint32_t acc_step = static_cast<uint32_t>(p.acc_chunks * slot_bytes) >> 4;
-      const uint32_t full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
-      const uint32_t tfull_a = smem_u32(tfull_bar), tempty_a = smem_u32(tempty_bar);
-      const int ksteps = p.P / 16;
-      const int num_units = p.num_units, iters_per_chunk = p.iters_per_chunk, iters_total = p.iters_total, stages = p.stages;
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t uphase = 0;
-      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-        const int pxc = unit / combos;
-        const int it0 = pxc * iters_per_chunk;
-        const int it1 = min(it0 + iters_per_chunk, iters_total);
-        mbar_wait_u32(tempty_a, uphase ^ 1);
-        tc_fence_after();
-        for (int it = it0; it < it1; ++it) {
-          mbar_wait_u32(full0 + stage * 8, phase);
-          tc_fence_after();
-          const uint64_t da_s = da0 + stage * stage_step;
-          const uint64_t db_s = db0 + stage * stage_step;
-          for (int ks = 0; ks < ksteps; ++ks) {
-            // 16 pixels = two 8-row swizzle atoms = 2048 B along the (slow) K dimension -> +128 in the address field
-            const uint32_t acc_flag = (it != it0 || ks != 0) ? 1u : 0u;
-            for (int a = 0; a < n_acc; ++a)
-              umma_bf16(tmem_base + a * acc_cols, da_s + ks * 128, db_s + a * acc_step + ks * 128, idesc, acc_flag);
-          }
-          umma_commit_u32(empty0 + stage * 8);
-          if (++stage == stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit_u32(tfull_a);
-        uphase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------------ epilogue: TMEM -> vector atomics
-    const int ew = warp - 4;
-    const int row = ew * 32 + lane;
-    uint32_t uphase = 0;
-    for (int unit = blockIdx.x; unit < p.num_units; unit += gridDim.x) {
-      const int pxc = unit / combos;
-      const int combo = unit - pxc * combos;
-      const int cob = combo / p.groups;
-      const int g = combo - cob * p.groups;
-      const int r = g / p.cgroups;
-      const int cbg = g - r * p.cgroups;
-      const int co = cob * 128 + row;
-      mbar_wait(tfull_bar, uphase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16);
-      for (int j = 0; j < p.G; ++j) {
-        const int cbi = j / p.S;
-        const int s = j - cbi * p.S;
-        const int tap = r * p.S + s;
-        const int ci0 = (cbg * p.cb_per_group + cbi) * 64;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(taddr + j * 64 + h * 32, v);
-          tmem_ld_wait();
-          if (co < p.cout) {
-            float4* dst = reinterpret_cast<float4*>(p.dw + (static_cast<size_t>(tap) * p.cout + co) * p.cin + ci0 + h * 32);
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              float4 f = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]),
-                                     __uint_as_float(v[4 * q + 2]), __uint_as_float(v[4 * q + 3]));
-              atomicAdd(dst + q, f);
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar);
-      uphase ^= 1;
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // -------------------------------------------------------------------- consumers: warpgroup wg <-> co chunk wg
+  const int wg = warp >> 2;
+  const bool active = wg < p.a_chunks;  // Cout == 64: warpgroup 1 only releases the stages
+  const int rrow = (warp & 3) * 16 + (lane >> 2);  // accumulator rows rrow, rrow + 8 (output channels within the chunk)
+  const int cq = (lane & 3) * 2;
+  // A = dY chunk wg (M = 64 co, MN-major, one 64-wide chunk); B = the G X chunks (N = 64 G ci, MN-major, chunks one slot
+  // apart = LBO).  16 pixels = two 8-row swizzle atoms = 2048 B along the (slow) K dimension -> +128 in the address field.
+  const uint64_t da0 = gmma_desc_sw128(smem_u32(smem) + wg * slot_bytes, slot_bytes, 1024);
+  const uint64_t db0 = gmma_desc_sw128(smem_u32(smem) + p.a_chunks * slot_bytes, slot_bytes, 1024);
+  const uint32_t stage_step = static_cast<uint32_t>(stage_bytes) >> 4;
+  const uint32_t full0 = smem_u32(full_bar);
+  const int ksteps = p.P / 16;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int unit = blockIdx.x; unit < p.num_units; unit += gridDim.x) {
+    const int pxc = unit / combos;
+    const int combo = unit - pxc * combos;
+    const int cob = combo / p.groups;
+    const int g = combo - cob * p.groups;
+    const int r = g / p.cgroups;
+    const int cbg = g - r * p.cgroups;
+    const int it0 = pxc * p.iters_per_chunk;
+    const int it1 = min(it0 + p.iters_per_chunk, p.iters_total);
+    float acc[32 * G];
+#pragma unroll
+    for (int i = 0; i < 32 * G; ++i) acc[i] = 0.f;
+    fence_acc(acc);
+    int prev = -1;
+    for (int it = it0; it < it1; ++it) {
+      mbar_wait_u32(full0 + stage * 8, phase);
+      if (active) {
+        wgmma_fence();
+        const uint64_t da_s = da0 + stage * stage_step;
+        const uint64_t db_s = db0 + stage * stage_step;
+        for (int ks = 0; ks < ksteps; ++ks) wgrad_mma<G>(acc, da_s + ks * 128, db_s + ks * 128);
+        wgmma_commit();
+        wgmma_wait<1>();
+      }
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == p.stages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    if (active) wgmma_wait<0>();
+    fence_acc(acc);
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    if (!active) continue;
+    // ---------------------------------------------------------------- flush: registers -> vector atomics
+    const int co = cob * 128 + wg * 64 + rrow;
+#pragma unroll
+    for (int j = 0; j < G; ++j) {
+      const int cbi = j / p.S;
+      const int s = j - cbi * p.S;
+      const int tap = r * p.S + s;
+      const int ci0 = (cbg * p.cb_per_group + cbi) * 64;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float2* dst = reinterpret_cast<float2*>(p.dw + (static_cast<size_t>(tap) * p.cout + co + 8 * h) * p.cin + ci0 + cq);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const int i = j * 8 + q;
+          atomicAdd(dst + 4 * q, make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]));
+        }
+      }
+    }
   }
 }
 
 void wgrad_plan_launch(const WgradPlanRaw& pl, cudaStream_t s) {
-  static bool attr_set = false;
-  const int smem_bytes = pl.p.stages * (pl.p.a_chunks + pl.p.G) * pl.p.P * 128 + 256;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
-    if (e != cudaSuccess)
-      throw std::runtime_error(std::string("conv_wgrad: cudaFuncSetAttribute: ") + cudaGetErrorString(e));
-    attr_set = true;
+  const int smem_bytes = pl.p.stages * (pl.p.a_chunks + pl.p.G) * pl.p.P * 128 + 256 + 1024;
+  if (pl.p.G < 1 || pl.p.G > 4 || pl.p.stages < 1 || pl.p.stages > kWgMaxStages || smem_bytes > 232448)
+    throw std::runtime_error("conv_wgrad: plan out of range (G 1..4, stages <= 8, <= 227 KB)");
+  static bool attr_set[4] = {false, false, false, false};
+  auto launch = [&](auto kern) {
+    if (!attr_set[pl.p.G - 1]) {
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
+      if (e != cudaSuccess)
+        throw std::runtime_error(std::string("conv_wgrad: cudaFuncSetAttribute: ") + cudaGetErrorString(e));
+      attr_set[pl.p.G - 1] = true;
+    }
+    kern<<<pl.grid, kWgThreads, smem_bytes, s>>>(pl.tmDY, pl.tmX[0], pl.tmX[1], pl.tmX[2], pl.tmX[3], pl.p);
+  };
+  switch (pl.p.G) {
+    case 1: launch(conv_wgrad_kernel<1>); break;
+    case 2: launch(conv_wgrad_kernel<2>); break;
+    case 3: launch(conv_wgrad_kernel<3>); break;
+    default: launch(conv_wgrad_kernel<4>); break;
   }
-  conv_wgrad_kernel<<<pl.grid, 256, smem_bytes, s>>>(pl.tmDY, pl.tmX[0], pl.tmX[1], pl.tmX[2], pl.tmX[3], pl.p);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string("conv_wgrad launch: ") + cudaGetErrorString(e));
 }

@@ -37,7 +37,7 @@ __device__ __forceinline__ void ldf8(const float* p, float (&f)[8]) {
   f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
 
-static inline int grid_for(int64_t work, int threads, int max_blocks = 148 * 16) {
+static inline int grid_for(int64_t work, int threads, int max_blocks = 132 * 16) {
   int64_t b = (work + threads - 1) / threads;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;
@@ -213,7 +213,7 @@ bn_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ s
 
 // rows per loop iteration of the BatchNorm apply / backward-apply kernels (1, 2 or 4); see bn_apply_kernel
 static int g_bn_rows_unroll = 1;
-// 3 = per-kernel choice from the measured table (profiles/r2_bn_unroll_check.txt): 4 rows for the forward apply without /
+// 3 = per-kernel choice (benchmarks/bn_unroll_check.py measures the table): 4 rows for the forward apply without /
 // with an identity residual and for the mask-free backward apply, 2 rows for the backward apply that recomputes the ReLU mask,
 // 1 row for the apply with a second BatchNorm on the residual (more rows spill there)
 void set_bn_rows_unroll(int u) { g_bn_rows_unroll = (u == 2 || u == 3 || u == 4) ? u : 1; }
@@ -224,7 +224,7 @@ static inline int rows_grid(int64_t M, int C, int threads) {
   const int lanes = cvec < threads ? cvec : threads;
   const int rpb = threads / lanes;
   int64_t b = (M + rpb - 1) / rpb;
-  const int64_t cap = 148 * 16;
+  const int64_t cap = 132 * 16;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (int)b;
@@ -376,7 +376,7 @@ static void col_reduce_launch(int mode, const void* a, const void* g2, const voi
                               int C, cudaStream_t s) {
   const int threads = 256;
   int blocks = (int)((M + 31) / 32);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
   const int cvec = C / 8;
   const int lanes = cvec < threads ? cvec : threads;
@@ -903,7 +903,7 @@ __global__ void weight_prep_kernel(const float* __restrict__ w, __nv_bfloat16* _
   }
 }
 void weight_prep(const float* w, void* wf, void* wd, int taps, int cout, int cin, cudaStream_t s) {
-  weight_prep_kernel<<<grid_for((int64_t)taps * cout * cin, 256, 148 * 4), 256, 0, s>>>(
+  weight_prep_kernel<<<grid_for((int64_t)taps * cout * cin, 256, 132 * 4), 256, 0, s>>>(
       w, (__nv_bfloat16*)wf, (__nv_bfloat16*)wd, taps, cout, cin);
 }
 
@@ -950,7 +950,7 @@ weight_prep_batched_kernel(const float* __restrict__ params, __nv_bfloat16* __re
 }
 void weight_prep_batched(const float* params, void* wd, const int64_t* table, int layers, int64_t total_tiles,
                          cudaStream_t s) {
-  int64_t grid = total_tiles < 148 * 16 ? total_tiles : 148 * 16;
+  int64_t grid = total_tiles < 132 * 16 ? total_tiles : 132 * 16;
   if (grid < 1) grid = 1;
   weight_prep_batched_kernel<<<(int)grid, 256, 0, s>>>(params, (__nv_bfloat16*)wd, table, layers, total_tiles);
 }

@@ -1,5 +1,5 @@
 // Classifier-head and stem-tail kernels (SURVEY.md K11, K14, K15): the bandwidth-bound glue around the two GEMM-shaped
-// ends of the network.  The FC layer itself runs on the tcgen05 implicit-GEMM kernels (a 1x1 "convolution" over a 1x1
+// ends of the network.  The FC layer itself runs on the wgmma implicit-GEMM kernels (a 1x1 "convolution" over a 1x1
 // image, csrc/conv_igemm.cuh / conv_wgrad.cu); what lives here is everything the reference's Dense + softmax head
 // (P1/02:175) and MaxPool backward need besides the GEMMs:
 //   * softmax_ce_head: bf16 logits + fp32 bias -> loss, accuracy, bf16 dlogits (padded columns zero) in one pass;
@@ -135,13 +135,12 @@ void pack_stem_weight(const float* w, void* out, cudaStream_t s) {
 //   PASS 0:   sum_dz += dz, sum_dzy += dz * y          (per channel; one flush of atomics per CTA)
 //   PASS 1:   dy = cA*dz + cB*y + cC
 // v1 of this kernel GATHERED per input pixel (compare the saved argmax of up to four windows, per channel) and was
-// instruction-bound: ncu 327 M warp instructions per pass, DRAM 15 % (profiles/r2_ncu_stem_bwd_*_v1.txt) - slower than the
-// three-kernel path it replaced.  v2 SCATTERS: every window contributes its gradient to exactly ONE pixel (its argmax), so
+// instruction-bound - slower than the three-kernel path it replaced.  v2 SCATTERS: every window contributes its gradient to exactly ONE pixel (its argmax), so
 // a CTA builds the da tile of 16x16 pixels x 64 channels in shared memory (fp32, 64 KB) by read-modify-write:
 //   * a warp handles (window, 32-channel half); lane = channel, so the smem bank is the lane whatever pixel is hit;
 //   * windows are processed in four colour classes (row parity x column parity): windows of one class have disjoint 3x3
 //     footprints, so plain (non-atomic) updates are race-free inside a class; __syncthreads between classes
-//     (shared-memory fp32 atomicAdd is a CAS spin loop on sm_100a - ATOMS.CAST.SPIN - and would dominate);
+//     (a shared-memory fp32 atomicAdd per element would serialise colliding lanes and dominate);
 //   * then the pixel phase reads da from smem, y from global, and reduces / applies.
 constexpr int kPoolTile = 8;
 constexpr int kPoolWin = kPoolTile + 1;
@@ -297,7 +296,7 @@ void stem_pool_bn_bwd(int pass, const void* idx, const void* g1, const void* g2,
     attr_set = true;
   }
   const int tiles = N * (Ho / kPoolTile) * (Wo / kPoolTile);
-  int grid = 148 * 3;
+  int grid = 132 * 3;
   if (grid > tiles) grid = tiles;
   if (pass == 0)
     stem_pool_bn_bwd_kernel<0><<<grid, 256, kStemDaBytes, s>>>((const uint8_t*)idx, (const __nv_bfloat16*)g1,

@@ -1,6 +1,6 @@
 // GPU JPEG decode for the sharded loader (`make_dataset(decode='gpu')`): the reference decodes with tf.io.decode_jpeg inside the
-// tf.data pipeline (P1/03:182-189); on a B200 box the host cannot decode fast enough for even ONE GPU (profiles/README.md R2.8:
-// 32 PIL threads 4.6 k images/s, one B200 trains 14 k), so the JPEG bitstreams cross PCIe compressed and are decoded on the
+// tf.data pipeline (P1/03:182-189); a host's CPU decoders can fall behind even ONE GPU's training rate, so the JPEG
+// bitstreams cross PCIe compressed and are decoded on the
 // device: nvJPEG (library, like cuDNN is for the baseline) with the HARDWARE backend (the NVJPG engines - no SM time, no CPU
 // Huffman decode) when the GPU has them, the GPU-hybrid backend otherwise; every image lands interleaved RGB in ONE scratch
 // buffer and OUR batched resize kernel (jpeg_resize.cu) writes the [n, H, W, 3] uint8 batch the stem kernels read.

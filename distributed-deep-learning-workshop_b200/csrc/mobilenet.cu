@@ -1,7 +1,7 @@
 // Kernels the reference's own model needs beyond the implicit-GEMM convolutions (SURVEY.md C14: frozen MobileNetV2 base +
 // GAP + Dropout + Dense, P1/03:159-178): the 3-channel 3x3/2 stem and the depthwise 3x3 convolutions, both with the
 // (inference-mode, i.e. folded) BatchNorm affine and ReLU6 applied in the same pass.  The pointwise (1x1) convolutions -
-// ~95 % of MobileNetV2's FLOPs - run on the tcgen05 kernels with the kStats = 4 epilogue (csrc/conv_igemm.cuh).
+// ~95 % of MobileNetV2's FLOPs - run on the wgmma kernels with the kStats = 4 epilogue (csrc/conv_igemm.cuh).
 // Activations are NHWC bf16 with the channel count padded to a multiple of 64 (the GEMM's K / N granularity); padded
 // channels are zero everywhere (zero weights, zero shift), so they never need special handling.
 #include <cuda_bf16.h>
@@ -80,7 +80,7 @@ void mbv2_stem(const uint8_t* x, const float* w, const float* scale, const float
                int ldc, float mul, float add, cudaStream_t s) {
   const int64_t total = (int64_t)N * (H / 2) * (W / 2) * 4;
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   mbv2_stem_kernel<<<(int)blocks, 256, 0, s>>>(x, w, scale, shift, (__nv_bfloat16*)out, N, H, W, ldc, mul, add);
 }
 
@@ -227,7 +227,7 @@ void dwconv3x3(const void* x, const float* w, const float* scale, const float* s
   if (tile_w == 4) {
     const int64_t total = (int64_t)N * Ho * ((Wo + 3) / 4) * (C / 8);
     int64_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
     if (stride == 1)
       dwconv3x3_tiled_kernel<1, 4><<<(int)blocks, 256, 0, s>>>((const __nv_bfloat16*)x, w, scale, shift, (__nv_bfloat16*)out, N, H, W, C, Ho, Wo);
@@ -237,7 +237,7 @@ void dwconv3x3(const void* x, const float* w, const float* scale, const float* s
   }
   const int64_t total = (int64_t)N * Ho * Wo * (C / 8);
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   if (stride == 1)
     dwconv3x3_kernel<1><<<(int)blocks, 256, 0, s>>>((const __nv_bfloat16*)x, w, scale, shift, (__nv_bfloat16*)out, N, H, W, C, Ho, Wo);

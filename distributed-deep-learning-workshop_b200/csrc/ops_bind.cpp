@@ -371,7 +371,7 @@ void cast_bf16(Tensor x, Tensor out) {
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   namespace py = pybind11;
-  m.doc() = "b200ddl bandwidth-bound sm_100a kernels and fused optimizers";
+  m.doc() = "b200ddl bandwidth-bound sm_90a kernels and fused optimizers";
   m.def("bn_finalize", &bn_finalize);
   m.def("bn_apply", &bn_apply, py::arg("y"), py::arg("scale"), py::arg("shift"), py::arg("res") = c10::nullopt,
         py::arg("res_scale") = c10::nullopt, py::arg("res_shift") = c10::nullopt, py::arg("out"), py::arg("relu") = true,

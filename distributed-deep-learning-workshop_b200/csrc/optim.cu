@@ -99,7 +99,7 @@ __global__ void cast_kernel(const float* __restrict__ x, __nv_bfloat16* __restri
 
 static inline int blocks_for(int64_t n4) {
   int64_t b = (n4 + 255) / 256;
-  if (b > 148 * 8) b = 148 * 8;
+  if (b > 132 * 8) b = 132 * 8;
   if (b < 1) b = 1;
   return (int)b;
 }

@@ -1,4 +1,4 @@
-// pybind layer of the hardware probes (csrc/umma_probe.cu, csrc/tma_probe.cu): measurement tools the kernel design rests
+// pybind layer of the hardware probe (csrc/tma_probe.cu): a measurement tool the kernel design rests
 // on, kept OUT of the hot-path extension (_b200_conv) - they are built as their own module, _b200_probe.
 #include <ATen/cuda/CUDAContext.h>
 #include <torch/extension.h>
@@ -57,29 +57,10 @@ static void tma_probe(at::Tensor x, int64_t rows_2d, int64_t bw, int64_t bh, int
   tma_probe_launch(tm, p, grid > 0 ? (int)grid : sm_count(), at::cuda::getCurrentCUDAStream());
 }
 
-// hardware probe (see csrc/umma_probe.cu): T [rows <= 256, 64] bf16, B [64, 64] bf16 -> out fp32 [128, 64]
-// out[8g + r] = T[shift + g * (sbo_bytes / 128) + r] . B^T
-static at::Tensor umma_probe(at::Tensor T, at::Tensor B, int64_t shift, bool use_base_offset, int64_t sbo_bytes) {
-  TORCH_CHECK(T.is_cuda() && T.scalar_type() == at::kBFloat16 && T.is_contiguous() && T.dim() == 2 && T.size(1) == 64);
-  TORCH_CHECK(B.is_cuda() && B.scalar_type() == at::kBFloat16 && B.is_contiguous() && B.size(0) == 64 && B.size(1) == 64);
-  const int64_t rows = T.size(0);
-  TORCH_CHECK(rows >= 136 && rows <= 256 && rows % 8 == 0, "T must have 136..256 rows");
-  TORCH_CHECK(sbo_bytes >= 128 && sbo_bytes % 128 == 0 && sbo_bytes < (1 << 18));
-  TORCH_CHECK(shift >= 0 && shift + 15 * (sbo_bytes / 128) + 8 <= rows, "the 16 row groups must stay inside T");
-  auto out = at::zeros({128, 64}, T.options().dtype(at::kFloat));
-  CUtensorMap tmT = map_2d(T.data_ptr(), rows, 64, 64, 64, (int)rows);
-  CUtensorMap tmB = map_2d(B.data_ptr(), 64, 64, 64, 64, 64);
-  umma_probe_launch(tmT, tmB, out.data_ptr<float>(), (int)shift, use_base_offset ? 1 : 0, (int)rows, (int)sbo_bytes,
-                    at::cuda::getCurrentCUDAStream());
-  return out;
-}
-
 }  // namespace b200
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   namespace py = pybind11;
-  m.doc() = "b200ddl hardware probes: UMMA descriptor addressing, TMA load-pipeline throughput (sm_100a)";
-  m.def("umma_probe", &b200::umma_probe, py::arg("T"), py::arg("B"), py::arg("shift"), py::arg("use_base_offset"),
-        py::arg("sbo_bytes") = 1024);
+  m.doc() = "b200ddl hardware probe: TMA load-pipeline throughput (sm_90a)";
   m.def("tma_probe", &b200::tma_probe);
 }

@@ -5,11 +5,11 @@
 // (L1/L2 resident), apply the input normalisation (x/127.5 - 1: the reference's `preprocess_input`, C13), convert
 // to bf16 and write a [128 pixels x 192 k] tile into shared memory in the canonical SWIZZLE_128B layout
 // (3 k-blocks of 128 rows x 128 B).  That single tile is
-//   * the K-major A operand of the forward GEMM   y[px, co]  = sum_k patch[px, k] * W[co, k]      (tcgen05, M=128, N=64)
+//   * the K-major A operand of the forward GEMM   y[px, co]  = sum_k patch[px, k] * W[co, k]   (wgmma, 2 x M=64, N=64)
 //   * the MN-major B operand of the weight-gradient GEMM  dW[co, k] = sum_px dy[px, co] * patch[px, k]  (N=192)
 // so the preprocess kernel, the bf16 copy of the input and cuDNN's padded-NHWC stem kernels all disappear.
-// Forward fuses the BatchNorm statistics like conv_igemm.cuh; wgrad keeps its 64x192 fp32 accumulator in TMEM for
-// the CTA's whole pixel range and flushes once with atomics.
+// Forward fuses the BatchNorm statistics like conv_igemm.cuh; wgrad keeps its 64x192 fp32 accumulator in the registers
+// of one warpgroup for the CTA's whole pixel range and flushes once with atomics.
 #include <stdexcept>
 #include <string>
 
@@ -18,7 +18,6 @@
 
 namespace b200 {
 
-constexpr int kStemK = 192;        // 147 padded to 3 x 64
 constexpr int kStemStages = 3;
 constexpr int kStemTileBytes = 3 * 128 * 128;  // 48 KB im2col tile
 constexpr int kPatchRowMax = 16 + 256 * 3 + 16;
@@ -163,27 +162,26 @@ __device__ __forceinline__ void stem_builder_loop(const StemParams& p, uint8_t* 
 }
 
 // ------------------------------------------------------------------------------------------------ forward
+// warps 0-7: two consumer warpgroups (wgmma rows 64g .. 64g+63 of the tile + epilogue), warps 8-15: im2col builders
+constexpr int kStemFwdThreads = 512;
 struct StemFwdSmem {
   static constexpr int kB = 3 * 64 * 128;            // weights: 3 k-blocks of [64 co x 64 k]
   static constexpr int kStaging = 2 * 128 * 128;
-  static constexpr int kTotal = kStemStages * kStemTileBytes + kB + kStaging + 256 + 2 * 64 * 4 + 2 * kPatchBytes;
+  static constexpr int kTotal = kStemStages * kStemTileBytes + kB + kStaging + 256 + 2 * 64 * 4 + 2 * kPatchBytes + 1024;
 };
 
-__global__ void __launch_bounds__(512, 1)
+__global__ void __launch_bounds__(kStemFwdThreads, 1)
 stem_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmY,
                 const __grid_constant__ StemParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = align_smem_1024(smem_raw);
   uint8_t* sA = smem;
   uint8_t* sB = smem + kStemStages * kStemTileBytes;
   uint8_t* sStage = sB + StemFwdSmem::kB;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sStage + StemFwdSmem::kStaging);
   uint64_t* full_bar = bars;                // [3]  builders -> MMA
   uint64_t* empty_bar = bars + 3;           // [3]  MMA -> builders
-  uint64_t* tfull_bar = bars + 6;           // [2]
-  uint64_t* tempty_bar = bars + 8;          // [2]
-  uint64_t* w_bar = bars + 10;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 11);
+  uint64_t* w_bar = bars + 6;
   float* sStat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [2][64]
   uint8_t* sPatch = reinterpret_cast<uint8_t*>(sStat) + 2 * 64 * 4;
 
@@ -194,11 +192,7 @@ stem_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
     tma_prefetch_desc(&tmY);
     for (int i = 0; i < kStemStages; ++i) {
       mbar_init(&full_bar[i], 8);   // one arrival per builder warp
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 4);
+      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
     mbar_init(w_bar, 1);
     fence_barrier_init();
@@ -208,88 +202,71 @@ stem_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
   for (int i = threadIdx.x; i < kStemStages * kStemTileBytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(sA)[i] = make_uint4(0u, 0u, 0u, 0u);
   for (int i = threadIdx.x; i < 2 * kPatchBytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(sPatch)[i] = make_uint4(0u, 0u, 0u, 0u);
   fence_proxy_async_smem();
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 128);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0 && lane == 0) {
-    // weights stay resident for the whole kernel
-    mbar_arrive_expect_tx(w_bar, StemFwdSmem::kB);
-    for (int kb = 0; kb < 3; ++kb) tma_load_2d(sB + kb * (64 * 128), &tmW, w_bar, kb * 64, 0);
-  } else if (warp == 1 && lane == 0) {
-    constexpr uint32_t idesc = umma_idesc_bf16(128, 64, 0, 0);
-    mbar_wait(w_bar, 0);
-    int stage = 0, acc = 0;
-    uint32_t phase = 0, acc_phase = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      const uint32_t d = tmem_base + acc * 64;
-#pragma unroll
-      for (int kb = 0; kb < 3; ++kb) {
-        const uint64_t da = umma_desc_sw128(smem_u32(sA + stage * kStemTileBytes + kb * (128 * 128)), 16, 1024);
-        const uint64_t db = umma_desc_sw128(smem_u32(sB + kb * (64 * 128)), 16, 1024);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16(d, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-      }
-      umma_commit(&empty_bar[stage]);
-      umma_commit(&tfull_bar[acc]);
-      if (++stage == kStemStages) { stage = 0; phase ^= 1; }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+  if (warp < 8) {
+    // ---------------------------------------------------------------- consumers: wgmma + epilogue (256 threads)
+    const int ctid = threadIdx.x;
+    const int wg = warp >> 2;
+    const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // accumulator rows row0, row0 + 8 (output pixel wo)
+    if (ctid == 0) {
+      // weights stay resident for the whole kernel
+      mbar_arrive_expect_tx(w_bar, StemFwdSmem::kB);
+      for (int kb = 0; kb < 3; ++kb) tma_load_2d(sB + kb * (64 * 128), &tmW, w_bar, kb * 64, 0);
     }
-  } else if (warp >= 4 && warp < 8) {
-    // ---------------------------------------------------------------- epilogue: TMEM -> bf16 -> TMA store (+ stats)
-    const int ew = warp - 4;
-    const int row = ew * 32 + lane;
-    const int etid = threadIdx.x - 128;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    mbar_wait(w_bar, 0);
+    const uint64_t da0 = gmma_desc_sw128(smem_u32(sA) + wg * 64 * 128, 16, 1024);
+    const uint64_t db0 = gmma_desc_sw128(smem_u32(sB), 16, 1024);
+    int stage = 0;
+    uint32_t phase = 0;
     int ctr = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++ctr) {
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
+      float acc[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+      fence_acc(acc);
+      mbar_wait(&full_bar[stage], phase);
+      wgmma_fence();
+      const uint64_t da_s = da0 + static_cast<uint32_t>(stage * (kStemTileBytes >> 4));
+#pragma unroll
+      for (int kb = 0; kb < 3; ++kb) {
+        const uint64_t da = da_s + kb * ((128 * 128) >> 4);
+        const uint64_t db = db0 + kb * ((64 * 128) >> 4);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n64k16<0, 0>(acc, da + 2 * k, db + 2 * k);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == kStemStages) { stage = 0; phase ^= 1; }
+
+      // ---------------------------------------------------------------- epilogue: registers -> bf16 -> TMA store (+ stats)
       uint8_t* sbuf = sStage + (ctr & 1) * (128 * 128);
-      if (etid == 0) tma_store_wait_read<1>();
-      named_bar_sync(1, 128);
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * 64;
+      if (ctid == 0) tma_store_wait_read<1>();
+      named_bar_sync(1, 256);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr + h * 32, r);
-        tmem_ld_wait();
-        if (h == 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-        }
+      for (int j = 0; j < 8; ++j) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          uint4 v;
-          v.x = pack_bf16x2(__uint_as_float(r[8 * j + 0]), __uint_as_float(r[8 * j + 1]));
-          v.y = pack_bf16x2(__uint_as_float(r[8 * j + 2]), __uint_as_float(r[8 * j + 3]));
-          v.z = pack_bf16x2(__uint_as_float(r[8 * j + 4]), __uint_as_float(r[8 * j + 5]));
-          v.w = pack_bf16x2(__uint_as_float(r[8 * j + 6]), __uint_as_float(r[8 * j + 7]));
-          *reinterpret_cast<uint4*>(sbuf + row * 128 + (((h * 4 + j) ^ (row & 7)) << 4)) = v;
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          *reinterpret_cast<uint32_t*>(sbuf + row * 128 + ((j ^ (row & 7)) << 4) + (lane & 3) * 4) =
+              pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
       }
       fence_proxy_async_smem();
-      named_bar_sync(2, 128);
-      if (etid == 0) {
+      named_bar_sync(1, 256);
+      if (ctid == 0) {
         tma_store_2d(&tmY, sbuf, 0, tile * p.Wo);
         tma_store_commit();
       }
       if (p.stat_sum != nullptr) {
-        const int cp = etid & 31, rg = etid >> 5;
+        const int cp = ctid & 31, rg = ctid >> 5;
         float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-        const int r_end = min(rg * 32 + 32, p.Wo);
+        const int r_end = min(rg * 16 + 16, p.Wo);
 #pragma unroll 8
-        for (int r = rg * 32; r < r_end; ++r) {
+        for (int r = rg * 16; r < r_end; ++r) {
           const uint32_t w = *reinterpret_cast<const uint32_t*>(sbuf + r * 128 + (((cp >> 2) ^ (r & 7)) << 4) + ((cp & 3) << 2));
           const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
           s0 += f.x; s1 += f.y;
@@ -300,44 +277,37 @@ stem_fwd_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
         atomicAdd(&sStat[64 + cp * 2], q0);
         atomicAdd(&sStat[64 + cp * 2 + 1], q1);
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
     if (p.stat_sum != nullptr) {
-      named_bar_sync(3, 128);
-      if (etid < 64) atomicAdd(p.stat_sum + etid, sStat[etid]);
-      else atomicAdd(p.stat_sqsum + (etid - 64), sStat[etid]);
+      named_bar_sync(3, 256);
+      if (ctid < 64) atomicAdd(p.stat_sum + ctid, sStat[ctid]);
+      else if (ctid < 128) atomicAdd(p.stat_sqsum + (ctid - 64), sStat[ctid]);
     }
-    if (etid == 0) tma_store_wait_all<0>();
-  } else if (warp >= 8) {
+    if (ctid == 0) tma_store_wait_all<0>();
+  } else {
     // ---------------------------------------------------------------- im2col builders (256 threads)
     const int bt = threadIdx.x - 256;
     const int n_my = blockIdx.x < p.num_tiles ? (p.num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     stem_builder_loop<kStemTileBytes>(p, sA, sPatch, full_bar, empty_bar, n_my,
                                       [&](int i) { return (int)blockIdx.x + i * (int)gridDim.x; }, bt, lane);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ weight gradient
+// warps 0-3: one consumer warpgroup (M = 64 output channels), warps 4-11: im2col builders, warp 12: dY TMA producer
+constexpr int kStemWgThreads = 416;
 struct StemWgSmem {
   static constexpr int kStage = kStemTileBytes + 128 * 128;   // im2col tile + dY tile
-  static constexpr int kTotal = kStemStages * kStage + 256 + 2 * kPatchBytes;
+  static constexpr int kTotal = kStemStages * kStage + 256 + 2 * kPatchBytes + 1024;
 };
 
-__global__ void __launch_bounds__(512, 1)
+__global__ void __launch_bounds__(kStemWgThreads, 1)
 stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ StemParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = align_smem_1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStemStages * StemWgSmem::kStage);
   uint64_t* full_bar = bars;      // [3]  8 builder warps + TMA producer
-  uint64_t* empty_bar = bars + 3; // [3]
-  uint64_t* tfull_bar = bars + 6;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 7);
+  uint64_t* empty_bar = bars + 3; // [3]  4 consumer warps
   uint8_t* sPatch = reinterpret_cast<uint8_t*>(bars) + 256;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -345,85 +315,74 @@ stem_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     tma_prefetch_desc(&tmDY);
     for (int i = 0; i < kStemStages; ++i) {
       mbar_init(&full_bar[i], 9);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);
     }
-    mbar_init(tfull_bar, 1);
     fence_barrier_init();
   }
   // zero all stages: pixel rows >= Wo of both operands must be exact zeros (they are never written)
   for (int i = threadIdx.x; i < kStemStages * StemWgSmem::kStage / 16; i += blockDim.x) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
   for (int i = threadIdx.x; i < 2 * kPatchBytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(sPatch)[i] = make_uint4(0u, 0u, 0u, 0u);
   fence_proxy_async_smem();
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // contiguous tile range per CTA
   const int per = (p.num_tiles + gridDim.x - 1) / gridDim.x;
   const int t0 = blockIdx.x * per;
   const int t1 = min(t0 + per, p.num_tiles);
 
-  if (warp == 0 && lane == 0) {
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = t0; tile < t1; ++tile) {
-      mbar_wait(&empty_bar[stage], phase ^ 1);
-      mbar_arrive_expect_tx(&full_bar[stage], p.Wo * 128);
-      tma_load_2d(smem + stage * StemWgSmem::kStage + kStemTileBytes, &tmDY, &full_bar[stage], 0, tile * p.Wo);
-      if (++stage == kStemStages) { stage = 0; phase ^= 1; }
+  if (warp == 12) {
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = t0; tile < t1; ++tile) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[stage], p.Wo * 128);
+        tma_load_2d(smem + stage * StemWgSmem::kStage + kStemTileBytes, &tmDY, &full_bar[stage], 0, tile * p.Wo);
+        if (++stage == kStemStages) { stage = 0; phase ^= 1; }
+      }
     }
-  } else if (warp == 1 && lane == 0) {
-    const uint32_t idesc = umma_idesc_bf16(128, kStemK, 1, 1);
+  } else if (warp < 4) {
+    // A = dY tile [px][64 co] (M = co, MN-major), B = im2col tile, 3 chunks of [px][64 k] 16 KB apart (N = 192, MN-major);
+    // 16 pixels = two 8-row swizzle atoms = 2048 B along K
+    float acc[96];
+#pragma unroll
+    for (int i = 0; i < 96; ++i) acc[i] = 0.f;
+    fence_acc(acc);
+    const int ksteps = (p.Wo + 15) / 16;
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = t0; tile < t1; ++tile) {
       mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
+      wgmma_fence();
       const uint32_t b0 = smem_u32(smem + stage * StemWgSmem::kStage);
       const uint32_t a0 = b0 + kStemTileBytes;
-      const int ksteps = (p.Wo + 15) / 16;
-      for (int ks = 0; ks < ksteps; ++ks) {
-        const uint64_t da = umma_desc_sw128(a0 + ks * 2048, 0, 1024);              // 64 co; rows 64..127 mirror
-        const uint64_t db = umma_desc_sw128(b0 + ks * 2048, 128 * 128, 1024);      // 3 chunks of 64 k
-        umma_bf16(tmem_base, da, db, idesc, (tile != t0 || ks != 0) ? 1u : 0u);
-      }
-      umma_commit(&empty_bar[stage]);
+      for (int ks = 0; ks < ksteps; ++ks)
+        wgmma_m64n192k16<1, 1>(acc, gmma_desc_sw128(a0 + ks * 2048, 128 * 128, 1024),
+                               gmma_desc_sw128(b0 + ks * 2048, 128 * 128, 1024));
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == kStemStages) { stage = 0; phase ^= 1; }
     }
-    umma_commit(tfull_bar);
-  } else if (warp >= 4 && warp < 6) {
-    // rows 0..63 of the accumulator = output channels
     if (t1 > t0) {
-      mbar_wait(tfull_bar, 0);
-      tc_fence_after();
-      const int co = (warp - 4) * 32 + lane;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>((warp - 4) * 32) << 16);
-#pragma unroll 1
-      for (int c32 = 0; c32 < kStemK / 32; ++c32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + c32 * 32, v);
-        tmem_ld_wait();
+      // rows = output channels, columns = k = tap * 3 + c
+      const int co0 = warp * 16 + (lane >> 2);
+      const int cq = (lane & 3) * 2;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int k = c32 * 32 + i;
-          if (k < 147) atomicAdd(p.dw + ((k / 3) * 64 + co) * 3 + (k % 3), __uint_as_float(v[i]));
+      for (int i = 0; i < 24; ++i) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int k = i * 8 + cq + (e & 1);
+          const int co = co0 + 8 * (e >> 1);
+          if (k < 147) atomicAdd(p.dw + ((k / 3) * 64 + co) * 3 + (k % 3), acc[4 * i + e]);
         }
       }
     }
-  } else if (warp >= 8) {
-    const int bt = threadIdx.x - 256;
+  } else {
+    const int bt = threadIdx.x - 128;
     stem_builder_loop<StemWgSmem::kStage>(p, smem, sPatch, full_bar, empty_bar, t1 > t0 ? t1 - t0 : 0,
                                           [&](int i) { return t0 + i; }, bt, lane);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 
@@ -438,7 +397,7 @@ void stem_fwd_launch(const StemPlanRaw& pl, cudaStream_t s) {
           "stem_fwd attr");
     attr = true;
   }
-  stem_fwd_kernel<<<pl.grid, 512, StemFwdSmem::kTotal, s>>>(pl.tmW, pl.tmY, pl.p);
+  stem_fwd_kernel<<<pl.grid, kStemFwdThreads, StemFwdSmem::kTotal, s>>>(pl.tmW, pl.tmY, pl.p);
   check(cudaGetLastError(), "stem_fwd launch");
 }
 void stem_wgrad_launch(const StemPlanRaw& pl, cudaStream_t s) {
@@ -448,7 +407,7 @@ void stem_wgrad_launch(const StemPlanRaw& pl, cudaStream_t s) {
           "stem_wgrad attr");
     attr = true;
   }
-  stem_wgrad_kernel<<<pl.grid, 512, StemWgSmem::kTotal, s>>>(pl.tmY, pl.p);
+  stem_wgrad_kernel<<<pl.grid, kStemWgThreads, StemWgSmem::kTotal, s>>>(pl.tmY, pl.p);
   check(cudaGetLastError(), "stem_wgrad launch");
 }
 

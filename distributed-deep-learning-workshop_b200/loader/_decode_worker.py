@@ -3,8 +3,7 @@
 
 Why processes: PIL releases the GIL inside the JPEG decoder and the resampler, but the Python part of opening an image
 (marker parsing in JpegImagePlugin, BytesIO, the final array copy) holds it for ~0.2 ms per image - decode THREADS of one
-process top out at ~4.6 k images/s no matter how many cores there are (measured: 32 threads on a 128-core host,
-profiles/README.md R2.8), a third of what one B200 trains on.
+process top out at a few thousand images/s no matter how many cores there are - below what one GPU trains on.
 
 Protocol (binary frames over the authenticated unix socket, no pickling):
     request : int32[3 + n] = (H, W, n, len_0 .. len_{n-1})  followed by the n payloads back to back;  an EMPTY frame = exit

@@ -4,9 +4,9 @@
     build_model(dropout=0.5)                                            (P2/01:92, P2/02:116)
     build_model()                                                       (P2/03:125)
 
-`arch='resnet50'` (TARGET, default on a B200): the hand-scheduled sm_100a engine, fully trainable, bf16.
+`arch='resnet50'` (TARGET, default on an H100): the hand-scheduled sm_90a engine, fully trainable, bf16.
 `arch='mobilenetv2'` (REF parity): frozen MobileNetV2 base + GAP + Dropout + Dense head - on a GPU the native
-`MobileNetV2Engine` (depthwise / stem kernels + tcgen05 pointwise convs with folded-BN epilogues), on CPU (or with
+`MobileNetV2Engine` (depthwise / stem kernels + wgmma pointwise convs with folded-BN epilogues), on CPU (or with
 `arch='mobilenetv2_torch'`, or `freeze_base=False`) the torch.nn module.
 `arch='resnet50_torch'`: torchvision-architecture ResNet-50 as a plain nn.Module (CPU plumbing runs).
 """

@@ -6,7 +6,7 @@ statistics), so every layer is convolution -> folded-BN affine -> ReLU6 [-> + re
 
   stem 3x3/2 (3 -> 32) from the uint8 batch      csrc/mobilenet.cu  mbv2_stem      (normalisation x/127.5-1 fused)
   depthwise 3x3 (stride 1 / 2)                    csrc/mobilenet.cu  dwconv3x3
-  pointwise 1x1 expand / project / last conv      csrc/conv_igemm.cuh, tcgen05 implicit GEMM with the kStats = 4 epilogue
+  pointwise 1x1 expand / project / last conv      csrc/conv_igemm.cuh, wgmma implicit GEMM with the kStats = 4 epilogue
                                                   (affine + ReLU6 / linear + residual add of the inverted-residual block)
   GAP + dropout, Dense head fwd / wgrad, CE       the same kernels as the ResNet-50 engine's head
 

@@ -1,9 +1,9 @@
-"""ResNet-50 as a hand-scheduled B200 engine (the TARGET model of BASELINE.json; reference model = C14).
+"""ResNet-50 as a hand-scheduled H100 engine (the TARGET model of BASELINE.json; reference model = C14).
 
-No autograd and no tracing compiler: forward and backward are explicit sequences of our sm_100a kernels over
+No autograd and no tracing compiler: forward and backward are explicit sequences of our sm_90a kernels over
 *static* NHWC bf16 buffers, so the whole training step is one CUDA graph.
 
-  conv            tcgen05/TMEM/TMA implicit GEMM (ops.conv.ConvForward) with the BatchNorm statistics reduced in
+  conv            wgmma/TMA implicit GEMM (ops.conv.ConvForward) with the BatchNorm statistics reduced in
                   the epilogue
   BN+ReLU(+add)   one bandwidth-bound pass (bn_apply); backward = reduce pass + apply pass (also emits the masked
                   skip-connection gradient)
@@ -98,15 +98,14 @@ class ResNet50Engine:
         # BatchNorm-backward reductions of bn1/bn2 computed inside the dgrad GEMM that produces their input gradient
         self.fuse_bwd_reduce = fuse_bwd_reduce
         # OPT-IN (B200DDL_FUSE_BN_COEFFS=1): BatchNorm scale/shift (forward) and A/B/C (backward) computed inside the apply
-        # kernels instead of 106 tiny launches.  Numerically equivalent (backward bit-identical), but MEASURED SLOWER:
-        # 19.39 vs 18.89 ms per step in an interleaved A/B at equal clocks (profiles/README.md 2.9) - a tiny dependent
-        # kernel costs only ~1.6 us of step time, the per-CTA coefficient recomputation in 106 streaming kernels more.
+        # kernels instead of 106 tiny launches.  Numerically equivalent (backward bit-identical); opt-in because the per-CTA
+        # coefficient recomputation in 106 streaming kernels can cost more than the tiny dependent launches it replaces.
         self.fuse_bn_coeffs = fuse_bn_coeffs or os.environ.get("B200DDL_FUSE_BN_COEFFS") == "1"
         # the gradient merge at every residual-block boundary (main path + skip path, ReLU mask, bn3 reduction) runs in
         # the epilogue of the next block's conv1 dgrad GEMM (conv_igemm kStats = 3); B200DDL_NO_BLOCK_GRAD=1 disables
         self.fuse_block_grad = (os.environ.get("B200DDL_NO_BLOCK_GRAD") != "1") if fuse_block_grad is None else bool(fuse_block_grad)
         # max-pool backward fused with the stem BatchNorm backward (csrc/head_stem.cu); B200DDL_STEM_BWD_FUSE=1 enables
-        # MEASURED SLOWER in its first version (profiles/README.md r2: 1,162 vs 884 us per step at batch 256), so opt-in:
+        # (opt-in):
         self.fuse_stem_bwd = (os.environ.get("B200DDL_STEM_BWD_FUSE") == "1") if fuse_stem_bwd is None else bool(fuse_stem_bwd)
         self._fused_reduce = set()
         self._block_fused = set()   # bn3 names whose reduction (and dz) come out of a fused dgrad epilogue
@@ -116,9 +115,8 @@ class ResNet50Engine:
         self._infer_fused = False
         # OPT-IN (B200DDL_TAILS=1): BatchNorm finalize / backward-coefficient computation in the LAST CTA of the GEMM that
         # accumulated the sums (conv_igemm last-CTA tails) instead of ~100 tiny dependent launches per step.  Numerically
-        # equivalent (gpu_check.py tails) but MEASURED SLOWER: 17.64 vs 17.11 ms per step, interleaved, both at 1965 MHz
-        # (profiles/r2_ab6_*.json): fence + ticket + a serial per-channel loop in ONE CTA at the end of every GEMM costs
-        # more than the ~4 us of a tiny dependent kernel that runs on all SMs.
+        # equivalent (gpu_check.py tails); opt-in because fence + ticket + a serial per-channel loop in ONE CTA at the end of
+        # every GEMM can cost more than a tiny dependent kernel that runs on all SMs.
         self.fuse_tails = os.environ.get("B200DDL_TAILS") == "1" and not self.fuse_bn_coeffs
         self._fin_fwd = set()    # BatchNorms finalized by their producing conv's tail (training mode)
         self._fin_bwd = set()    # BatchNorms whose backward coefficients come from a dgrad tail
@@ -522,7 +520,7 @@ class ResNet50Engine:
             x_in = A[b.name + ".out"]
         self.feat = x_in  # [N, 7, 7, 2048]
         self.pooled = torch.zeros(N, 2048, **bf)
-        # classifier head on the same tcgen05 kernels: a 1x1 "convolution" over a 1x1 image (reference Dense, P1/02:175)
+        # classifier head on the same wgmma kernels: a 1x1 "convolution" over a 1x1 image (reference Dense, P1/02:175)
         ncp = self.classes_padded
         self.logits16 = torch.zeros(N, ncp, **bf)
         self._fc_fwd = C.ConvForward(self.pooled.view(N, 1, 1, 2048), self.w16v("fc.weight"), self.logits16.view(N, 1, 1, ncp),
@@ -627,7 +625,7 @@ class ResNet50Engine:
         drop = self.dropout if training else 0.0
         self._drop_seed = self.seed * 1000003 + self._step_count
         e.gap_fwd(self.feat, self.pooled, drop, self._drop_seed)
-        self._fc_fwd.run()  # bf16 logits (class dimension padded) on the tcgen05 GEMM
+        self._fc_fwd.run()  # bf16 logits (class dimension padded) on the wgmma GEMM
         e.zero_(self.stats)
         # + bias, softmax cross-entropy, accuracy, bf16 dlogits (padded columns zero) in one kernel
         e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits,
@@ -704,7 +702,7 @@ class ResNet50Engine:
         e.zero_(self.grads)  # wgrad accumulates with atomics
         if self.fuse_bn_coeffs:
             e.zero_(self._bn_bwd_sums)  # sum(dz), sum(dz*y) of every layer; nobody zeroes them after use on the fused path
-        # classifier head: wgrad + dgrad on the tcgen05 GEMMs, bias gradient = column sums of dlogits
+        # classifier head: wgrad + dgrad on the wgmma GEMMs, bias gradient = column sums of dlogits
         self._fc_wg.run()
         e.fc_bias_grad(self.dlogits16, self.g("fc.bias"))
         self._fc_dg.run()

@@ -1,9 +1,9 @@
-"""Python entry points of the sm_100a kernels.
+"""Python entry points of the sm_90a kernels.
 
 ``ops.ext(name)`` loads (building in-tree if needed) one of the extensions:
 
-    _b200_conv    tcgen05/TMEM/TMA implicit-GEMM convolution forward / dgrad / wgrad
-    _b200_probe   hardware probes (UMMA descriptor addressing, TMA pipeline throughput); never on a hot path
+    _b200_conv    wgmma/TMA implicit-GEMM convolution forward / dgrad / wgrad
+    _b200_probe   hardware probe (TMA pipeline throughput); never on a hot path
     _b200_ops     BN / ReLU / pool / softmax-CE / preprocess kernels + fused optimizers
     _b200_comm    fused all-reduce kernels over NVLink symmetric memory
     _b200_loader  pinned-host ring buffer with side-stream H2D
@@ -19,7 +19,7 @@ EXT_NAMES = tuple(_build.EXTENSIONS)
 
 
 # Rows per loop iteration of the BatchNorm apply / backward-apply kernels (csrc/elementwise.cu): 1, 2 or 4, bit-identical
-# results; the default is the value the A/B in profiles/README.md R2.9 settled on, `B200DDL_BN_UNROLL` overrides it.
+# results; `B200DDL_BN_UNROLL` overrides the default.
 BN_ROWS_UNROLL_DEFAULT = 1
 
 
@@ -47,10 +47,10 @@ def require_native() -> None:
     import torch
 
     if not torch.cuda.is_available():
-        raise RuntimeError("b200ddl: this code path needs a CUDA device (B200, sm_100a)")
+        raise RuntimeError("b200ddl: this code path needs a CUDA device (H100, sm_90a)")
     cap = torch.cuda.get_device_capability()
-    if cap[0] != 10:
-        raise RuntimeError(f"b200ddl: kernels are compiled for sm_100a only, found sm_{cap[0]}{cap[1]}")
+    if cap != (9, 0):
+        raise RuntimeError(f"b200ddl: kernels are compiled for sm_90a only, found sm_{cap[0]}{cap[1]}")
 
 
 def kernel_launches() -> int:

@@ -1,11 +1,11 @@
-"""In-tree build + load of the sm_100a extensions.
+"""In-tree build + load of the sm_90a extensions.
 
-Every extension is compiled with ``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` straight into
+Every extension is compiled with ``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` straight into
 ``csrc/build/<name>/<name>.so`` (in-tree, so the binary travels to the GPU box with the repo snapshot) and is
 loaded by file path.  A content hash of the sources + flags is stored next to the ``.so``; when it matches, the
 binary is imported directly with no ninja/JIT step, which keeps GPU-box start-up to a dlopen.
 
-The reference has no native code at all (SURVEY.md §2.2); these extensions are the B200-native equivalents of
+The reference has no native code at all (SURVEY.md §2.2); these extensions are the H100-native equivalents of
 what it delegates to TF/cuDNN/Horovod/NCCL/Petastorm.
 """
 from __future__ import annotations
@@ -22,7 +22,7 @@ CSRC = os.path.normpath(os.path.join(os.path.dirname(os.path.abspath(__file__)),
 BUILD_ROOT = os.path.join(CSRC, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "--use_fast_math",
     "-U__CUDA_NO_HALF_OPERATORS__", "-U__CUDA_NO_HALF_CONVERSIONS__",
@@ -33,7 +33,7 @@ CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC"]
 # name -> sources (relative to csrc/)
 EXTENSIONS: Dict[str, List[str]] = {
     "_b200_conv": ["conv_igemm.cu", "conv_wgrad.cu", "stem.cu", "tmap.cpp", "conv_bind.cpp"],
-    "_b200_probe": ["umma_probe.cu", "tma_probe.cu", "tmap.cpp", "probe_bind.cpp"],   # hardware probes, not on any hot path
+    "_b200_probe": ["tma_probe.cu", "tmap.cpp", "probe_bind.cpp"],   # hardware probe, not on any hot path
     "_b200_ops": ["elementwise.cu", "head_stem.cu", "mobilenet.cu", "optim.cu", "ops_bind.cpp"],
     "_b200_comm": ["allreduce.cu", "comm_bind.cpp"],
     "_b200_loader": ["ring_loader.cpp"],

@@ -1,4 +1,4 @@
-"""Planning layer of the tcgen05 implicit-GEMM convolution (kernels: csrc/conv_igemm.cuh, csrc/conv_wgrad.cu).
+"""Planning layer of the wgmma implicit-GEMM convolution (kernels: csrc/conv_igemm.cuh, csrc/conv_wgrad.cu).
 
 A convolution on NHWC bf16 tensors is described to the kernels as
   * 1..4 *views* of the input that share one pixel grid (for stride 2 these are the four parity sub-grids
@@ -63,16 +63,12 @@ def halo_box(h: int, w: int, cin: int, cout: int, R: int, S: int, stride: int, p
 
     Halo mode (csrc/conv_igemm.cuh): 3x3 / stride 1 / pad 1 with a resident 64x64 filter; one [w x (bh+2)] load per
     horizontal tap offset serves the three vertical taps, so a stage (28 KB) must hold w * (bh + 2) <= 224 pixels and the
-    MMA tile w * bh <= 128.  `B200DDL_NO_HALO=1` keeps the generic boxes (A/B measurements)."""
+    MMA tile w * bh <= 128; the vertical taps start w and 2*w rows into the stage, which must be whole 8-row swizzle atoms
+    (w % 8 == 0).  `B200DDL_NO_HALO=1` keeps the generic boxes (A/B measurements)."""
     if os.environ.get("B200DDL_NO_HALO") == "1" or os.environ.get("B200DDL_NO_RESIDENT_FILTER") == "1":
         return None
-    if not (R == 3 and S == 3 and stride == 1 and pad == 1 and cin == 64 and cout == 64):
+    if not (R == 3 and S == 3 and stride == 1 and pad == 1 and cin == 64 and cout == 64 and w % 8 == 0):
         return None
-    if os.environ.get("B200DDL_HALO2D") == "1" and w % 8 == 0:
-        # two-dimensional halo (opt-in): 8-pixel-wide boxes, one [(8+2) x (bh+2)] load per tile serves all nine taps
-        cand = [bh for bh in _divisors(h) if bh <= 16 and 10 * (bh + 2) <= 224]
-        if cand:
-            return (8, max(cand), 1)
     best = None
     for bh in _divisors(h):
         if w * bh <= 128 and w * (bh + 2) <= 224:
@@ -299,14 +295,14 @@ class ConvWgrad:
         if flat:
             bw = bh = bn = 0
         else:
-            # keep >= 3 pipeline stages in 227 KB: stage = (dY chunks + X chunks) * P pixels * 128 B
+            # keep >= 3 pipeline stages in 227 KB: stage = (dY chunks + X chunks) * P pixels * 128 B (G <= 4 X chunks)
             cin, cout = x.shape[3], dy.shape[3]
             cb = cin // 64
-            g = S * (2 if (cb >= 2 and S * 2 <= 6) else 1) if S > 1 else max(d for d in (1, 2, 3, 4) if cb % d == 0)
+            g = S * (2 if (cb >= 2 and S * 2 <= 4) else 1) if S > 1 else max(d for d in (1, 2, 3, 4) if cb % d == 0)
             chunks = (1 if cout == 64 else 2) + g
             budget = smem_budget if 0 < smem_budget < 232448 else 232448
             want_stages = 3 if budget >= 200000 else 2
-            rows = min(128, ((budget - 256) // (want_stages * chunks * 128)) // 16 * 16)
+            rows = min(128, ((budget - 256 - 1024) // (want_stages * chunks * 128)) // 16 * 16)
             bw, bh, bn = pick_box(N, Ho, Wo, rows=rows, multiple_of=16)
         self.box = (bw, bh, bn)
         self.plan = ext.WgradPlan(dy, taps.views, dw, R, S, taps.tap_map, taps.tap_dw, taps.tap_dh, bw, bh, bn,

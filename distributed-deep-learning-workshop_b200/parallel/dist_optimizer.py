@@ -42,25 +42,17 @@ class DistributedOptimizer:
         # The LAST bucket to complete is the only all-reduce nothing can hide (backward has ended): keep it small.  The
         # final `tail_mb` of the gradient buffer (the layers that finish last: stem + first stage) become their own bucket.
         self.tail_bytes = int(tail_mb * 2 ** 20)
-        # 'auto' picks the kernel PER BUCKET from the measured sweeps (profiles/): the P2P two-shot wins below ~32 MB
-        # (8 GPUs, 16 MB: 92 vs 115 us), the in-switch NVLS reduction above
-        # measured crossover (profiles/r2_allreduce_w{2,4,8}.log, 16 MB bucket): 2 GPUs P2P 43 us vs NVLS 56; 4 GPUs NVLS 55 vs
-        # P2P 62-76 -> with 2 ranks P2P always, with more ranks NVLS from 1 MB up (the in-switch reduction needs few CTAs:
-        # 8-16 are as fast as 64, so NVLS buckets use `nvls_blocks`)
+        # 'auto' picks the kernel PER BUCKET: with 2 ranks the P2P two-shot always, with more ranks the in-switch NVLS
+        # reduction from 1 MB up (it needs few CTAs, so NVLS buckets use `nvls_blocks`).  `benchmarks/allreduce_check.py`
+        # sweeps both against NCCL to check the crossover on a given box.
         if nvls_min_mb is None:
-            # 4 / 8 ranks: NVLS also wins below 1 MB in the sweeps (1 KB: 15.7 vs 18.8 us / 15.4 vs 25.9; 1 MB: 19.9 vs 24.0 /
-            # 19.8 vs 31.5), i.e. `nvls_min_mb=0` would save ~10 us of the exposed tail bucket; the shipped default stays
-            # at the configuration the 4- and 8-GPU training runs were MEASURED with (profiles/r2_bench_w{4,8}.json)
             nvls_min_mb = 1e9 if core.size() <= 2 else 1.0
         self.nvls_min_bytes = int(nvls_min_mb * 2 ** 20)
-        # 8 GPUs, 16 MB (profiles/r2_allreduce_sweep_w8.json): 8 CTAs 51.8 us, 16: 57.9, 32: 64.9 - each rank only reduces
-        # 1/world of the bucket, so the more ranks the fewer CTAs saturate the switch's reduction path.  `nvls_blocks=8` is the
-        # faster setting for the isolated kernel at 8 ranks; the default (16) is what the measured training runs used.
+        # each rank only reduces 1/world of the bucket, so the more ranks the fewer CTAs saturate the switch's reduction path
         self.nvls_blocks = nvls_blocks if nvls_blocks is not None else 16
         self.overlap = overlap
         self.algo = algo
-        # CTAs of a comm kernel (512 threads each).  16 MB bucket, 2 GPUs, two-shot P2P: 8 CTAs 121 us, 16: 67, 32: 43, 64: 40
-        # (profiles/r2_allreduce_w2.log) - 32 is where the curve flattens; they occupy SM slots only while a bucket is in flight
+        # CTAs of a comm kernel (512 threads each); they occupy SM slots only while a bucket is in flight
         self.comm_blocks = comm_blocks
         self.average = average
         # fused_update: reduce-scatter + SGD-momentum update of my 1/N slice + multicast of the new fp32/bf16 weights

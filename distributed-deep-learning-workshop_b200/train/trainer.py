@@ -1,7 +1,7 @@
 """Trainer: the Keras `compile / fit / evaluate / predict` surface of the reference (P1/02:194-215,
 P1/03:204-234,325-358, P2/03:206) on top of two execution backends:
 
-* **engine backend** - `models.ResNet50Engine`: hand-scheduled sm_100a kernels, whole step in one CUDA graph,
+* **engine backend** - `models.ResNet50Engine`: hand-scheduled sm_90a kernels, whole step in one CUDA graph,
   gradients born inside the (symmetric) flat buffer that `DistributedOptimizer` all-reduces while backward runs;
 * **module backend** - any `torch.nn.Module` (e.g. the reference's frozen MobileNetV2 + Dense head, or CPU runs):
   autograd computes gradients into the same kind of flat buffer (`FlatParams`), so optimizers, callbacks and the
@@ -457,7 +457,7 @@ class Trainer:
         if _is_engine(self.model):
             n = self.model.num_parameters()
             tr = self.model.trainable_parameters() if hasattr(self.model, "trainable_parameters") else n
-            lines = [f"Model: {self.model.arch} (B200 engine)", f"Total params: {n:,}", f"Trainable params: {tr:,}"]
+            lines = [f"Model: {self.model.arch} (H100 engine)", f"Total params: {n:,}", f"Trainable params: {tr:,}"]
             if tr != n:
                 lines.append(f"Non-trainable params: {n - tr:,}")
         else:

@@ -3,10 +3,9 @@ import os
 
 
 def usable_cpus() -> int:
-    """CPUs this process may actually USE: the smaller of the affinity mask and the cgroup CPU quota.  On the B200 pods
-    `os.cpu_count()` says 128 while the container's quota (`cpu.max` = "1600000 100000") is 16 CPUs - sizing a decode pool
-    by the former oversubscribes 8x and LOSES throughput (32 processes 6.5 k images/s, 120 processes 4.2 k;
-    profiles/r2_cpu_decode_scaling.txt)."""
+    """CPUs this process may actually USE: the smaller of the affinity mask and the cgroup CPU quota.  In a container
+    `os.cpu_count()` can report every host core while the quota (`cpu.max`, e.g. "1600000 100000") allows 16 - sizing a
+    decode pool by the former oversubscribes it and loses throughput."""
     try:
         n = len(os.sched_getaffinity(0))
     except (AttributeError, OSError):

@@ -1,7 +1,7 @@
 """Part 1 / 03_model_training_distributed  (reference: 03_model_training_distributed.py) - the main path.
 
 converter (sharded loader) -> `train_and_evaluate_hvd()` per rank -> Runner(np).run(...) -> rank 0 logs + returns.
-On an 8xB200 box set HVD_NP=8: the gradient all-reduce inside DistributedOptimizer is our fused NVLS/P2P kernel."""
+On an 8xH100 box set HVD_NP=8: the gradient all-reduce inside DistributedOptimizer is our fused NVLS/P2P kernel."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from common import *  # noqa: F401,F403

@@ -19,7 +19,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with `pytest -m gpu` on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with `pytest -m gpu` on the GPU box")
 
 
 def pytest_collection_modifyitems(config, items):

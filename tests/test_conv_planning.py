@@ -54,13 +54,15 @@ def test_weight_layout_roundtrip():
 
 
 def test_halo_box_selection(monkeypatch):
-    """Full-width single-image boxes only for the 3x3 / stride-1 / 64->64 layers whose box + halo fits one 28 KB stage."""
+    """Full-width single-image boxes only for the 3x3 / stride-1 / 64->64 layers whose box + halo fits one 28 KB stage and
+    whose width is a multiple of 8 (the vertical taps start whole 8-row swizzle atoms into the stage)."""
     from b200ddl.ops import conv as C
 
     monkeypatch.delenv("B200DDL_NO_HALO", raising=False)
     monkeypatch.delenv("B200DDL_NO_RESIDENT_FILTER", raising=False)
     assert C.halo_box(56, 56, 64, 64, 3, 3, 1, 1) == (56, 2, 1)      # 112-pixel tile, 224-pixel halo stage
-    assert C.halo_box(28, 28, 64, 64, 3, 3, 1, 1) == (28, 4, 1)
+    assert C.halo_box(24, 24, 64, 64, 3, 3, 1, 1) == (24, 4, 1)
+    assert C.halo_box(28, 28, 64, 64, 3, 3, 1, 1) is None            # 28-row tap offsets are not whole swizzle atoms
     assert C.halo_box(56, 56, 128, 128, 3, 3, 1, 1) is None          # filter does not fit resident
     assert C.halo_box(56, 56, 64, 64, 3, 3, 2, 1) is None            # strided
     assert C.halo_box(56, 56, 64, 64, 1, 1, 1, 0) is None
