@@ -307,6 +307,7 @@ struct ConvPlan {
     ++launches;
   }
   int grid() const { return raw.grid; }
+  int tiles() const { return raw.p.num_tiles; }
   int block_n() const { return raw.block_n; }
   int res_b() const { return raw.res_b; }
   int halo() const { return raw.halo; }
@@ -415,6 +416,9 @@ struct WgradPlan {
   int grid() const { return raw.grid; }
   int units() const { return raw.p.num_units; }
   int stages() const { return raw.p.stages; }
+  int G() const { return raw.p.G; }
+  int px_chunks() const { return raw.p.px_chunks; }
+  int mode() const { return raw.p.mode; }
 };
 
 struct StemPlan {
@@ -502,6 +506,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def_property_readonly("has_tail", &b200::ConvPlan::has_tail)
       .def_readonly("launches", &b200::ConvPlan::launches)
       .def_property_readonly("grid", &b200::ConvPlan::grid)
+      .def_property_readonly("tiles", &b200::ConvPlan::tiles)
       .def_property_readonly("block_n", &b200::ConvPlan::block_n)
       .def_property_readonly("resident_filter", &b200::ConvPlan::res_b)
       .def_property_readonly("halo", &b200::ConvPlan::halo)
@@ -516,7 +521,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def_readonly("launches", &b200::WgradPlan::launches)
       .def_property_readonly("grid", &b200::WgradPlan::grid)
       .def_property_readonly("units", &b200::WgradPlan::units)
-      .def_property_readonly("stages", &b200::WgradPlan::stages);
+      .def_property_readonly("stages", &b200::WgradPlan::stages)
+      .def_property_readonly("G", &b200::WgradPlan::G)
+      .def_property_readonly("px_chunks", &b200::WgradPlan::px_chunks)
+      .def_property_readonly("mode", &b200::WgradPlan::mode);
   py::class_<b200::StemPlan>(m, "StemPlan")
       .def(py::init<at::Tensor, c10::optional<at::Tensor>, at::Tensor, c10::optional<at::Tensor>,
                     c10::optional<at::Tensor>, c10::optional<at::Tensor>, double, double, int64_t>(),

@@ -185,12 +185,14 @@ class ConvDgrad:
         dz = (conv_transpose(dy, w) + skip_grad) * relu_mask - the complete masked gradient of the previous residual
         block's output - and sum(dz), sum(dz * y3) of that block's last BatchNorm are accumulated in the same epilogue.
         ``skip_grad`` has dx's grid, or its stride-2 sub-grid (compact gradient of a strided 1x1 projection)."""
-        ext = _build.load("_b200_conv")
-        self.R, self.S, self.stride, self.pad = R, S, stride, pad
-        self.fused_bwd_stats = bwd_stats is not None and stride == 1
-        self.block_grad = block_grad is not None
+        if bwd_stats is not None and stride != 1:
+            raise ValueError("bwd_stats: stride-1 convs only (a strided dgrad has no fused reduction)")
         if block_grad is not None and (stride != 1 or bwd_stats is not None):
             raise ValueError("block_grad: stride-1 convs only, and not together with bwd_stats")
+        ext = _build.load("_b200_conv")
+        self.R, self.S, self.stride, self.pad = R, S, stride, pad
+        self.fused_bwd_stats = bwd_stats is not None
+        self.block_grad = block_grad is not None
         self.w_master = w_master
         if wbufs is not None:
             assert wbuf is None and len(wbufs) == len(self.part_taps(R, S, stride, pad))
@@ -200,6 +202,7 @@ class ConvDgrad:
         taps_total, cout, cin = w_master.shape
         assert taps_total == R * S
         self.parts = []  # (plan, weight buffer, tap index list)
+        self.boxes = []  # pixel box (bw, bh, bn) of each part; (0, 0, 0) = flat
         self._idx_dev = {}
         self.needs_zero = False
         self.dx = dx
@@ -233,6 +236,7 @@ class ConvDgrad:
                 plan = ext.ConvPlan([dy], wbuf, dx, tm, dw, dh, box[0], box[1], box[2], None, None, max_ctas)
             _plans.add(plan)
             self.parts.append((plan, wbuf, idx))
+            self.boxes.append(box)
         else:
             # output parity classes: dx[2i+ph, 2j+pw] = sum_{taps with (r-pad)%2==ph, (s-pad)%2==pw} dy[i-dh, j-dw] w[r,s]
             for ph in range(2):
@@ -259,6 +263,7 @@ class ConvDgrad:
                     plan = ext.ConvPlan([dy], wbuf, out_view, tm, dw, dh, box[0], box[1], box[2], None, None, max_ctas)
                     _plans.add(plan)
                     self.parts.append((plan, wbuf, idx))
+                    self.boxes.append(box)
         self.refresh_weights()
 
     def refresh_weights(self) -> None:

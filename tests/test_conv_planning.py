@@ -53,6 +53,18 @@ def test_weight_layout_roundtrip():
     assert torch.equal(out[5, 3 * 17 + 2], ws[17, 5, 2]) and float(out[:, 147:].abs().sum()) == 0.0
 
 
+def test_dgrad_refuses_fused_reductions_when_strided():
+    """A stride-2 dgrad has no fused BatchNorm-backward reduction: asking for one is an error, not silently zero sums."""
+    dy = torch.zeros(1, 4, 4, 64, dtype=torch.bfloat16)
+    dx = torch.zeros(1, 8, 8, 64, dtype=torch.bfloat16)
+    w = torch.zeros(9, 64, 64)
+    z = torch.zeros(64)
+    with pytest.raises(ValueError, match="bwd_stats: stride-1"):
+        C.ConvDgrad(dy, w, dx, 3, 3, 2, 1, bwd_stats=(dx, z, z, z.clone(), z.clone()))
+    with pytest.raises(ValueError, match="block_grad: stride-1"):
+        C.ConvDgrad(dy, w, dx, 3, 3, 2, 1, block_grad=(dx, z, dx, z.clone(), z.clone()))
+
+
 def test_halo_box_selection(monkeypatch):
     """Full-width single-image boxes only for the 3x3 / stride-1 / 64->64 layers whose box + halo fits one 28 KB stage and
     whose width is a multiple of 8 (the vertical taps start whole 8-row swizzle atoms into the stage)."""
