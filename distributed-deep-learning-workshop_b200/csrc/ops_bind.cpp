@@ -20,6 +20,26 @@ inline void chk(const Tensor& t, at::ScalarType ty, const char* name) {
   TORCH_CHECK(t.scalar_type() == ty, name, " has wrong dtype");
   TORCH_CHECK(t.is_contiguous(), name, " must be contiguous");
 }
+// The kernels move 16 bytes (8 bf16 / 4 fp32) per access, or 8 bytes for the uint8 argmax / bf16x4 stores.
+// Check messages are strings only: formatting an integer into a TORCH_CHECK message crashes this extension when
+// its libstdc++ differs from the one torch was built with.
+inline void aligned(const Tensor& t, int bytes, const char* name) {
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % bytes == 0, name,
+              " is not aligned for the kernel's vector accesses");
+}
+// contiguous CUDA tensor of dtype `ty` with n elements, `align`-byte aligned (1: the kernel reads it element-wise)
+inline void vec(const Tensor& t, at::ScalarType ty, int64_t n, const char* name, int align = 16) {
+  chk(t, ty, name);
+  TORCH_CHECK(t.numel() == n, name, " has the wrong number of elements");
+  aligned(t, align, name);
+}
+// bf16 NHWC / [M, C] activation: C % 8 == 0 and 16-byte aligned
+inline int act_channels(const Tensor& t, const char* name) {
+  chk(t, at::kBFloat16, name);
+  TORCH_CHECK(t.dim() >= 1 && t.size(-1) % 8 == 0 && t.size(-1) > 0, name, ": channel count must be a positive multiple of 8");
+  aligned(t, 16, name);
+  return (int)t.size(-1);
+}
 inline const float* fp(const OptT& t) { return t.has_value() ? t->data_ptr<float>() : nullptr; }
 inline const void* vp(const OptT& t) { return t.has_value() ? t->data_ptr() : nullptr; }
 inline void after() {
@@ -38,14 +58,24 @@ void bn_finalize(Tensor sum, Tensor sqsum, double count, Tensor gamma, Tensor be
   after();
 }
 
+// a bf16 tensor with the same element count as the activation `like`, 16-byte aligned
+inline void same_act(const Tensor& t, const Tensor& like, const char* name) {
+  chk(t, at::kBFloat16, name);
+  TORCH_CHECK(t.numel() == like.numel(), name, " must have as many elements as the activation");
+  aligned(t, 16, name);
+}
+
 void bn_apply(Tensor y, Tensor scale, Tensor shift, OptT res, OptT res_scale, OptT res_shift, Tensor out, bool relu,
               OptT mask) {
-  chk(y, at::kBFloat16, "y");
-  chk(out, at::kBFloat16, "out");
-  const int C = (int)y.size(-1);
+  const int C = act_channels(y, "y");
   const int64_t M = y.numel() / C;
-  TORCH_CHECK(C % 8 == 0 && scale.numel() == C && shift.numel() == C && out.numel() == y.numel());
-  if (res.has_value()) { chk(*res, at::kBFloat16, "res"); TORCH_CHECK(res->numel() == y.numel()); }
+  same_act(out, y, "out");
+  vec(scale, at::kFloat, C, "scale");
+  vec(shift, at::kFloat, C, "shift");
+  if (res.has_value()) same_act(*res, y, "res");
+  TORCH_CHECK(res_scale.has_value() == res_shift.has_value() && (!res_scale.has_value() || res.has_value()),
+              "res_scale and res_shift go together, and need res");
+  if (res_scale.has_value()) { vec(*res_scale, at::kFloat, C, "res_scale"); vec(*res_shift, at::kFloat, C, "res_shift"); }
   if (mask.has_value()) { chk(*mask, at::kByte, "mask"); TORCH_CHECK(mask->numel() * 8 == y.numel()); }
   b200::bn_apply(y.data_ptr(), scale.data_ptr<float>(), shift.data_ptr<float>(), vp(res), fp(res_scale),
                  fp(res_shift), out.data_ptr(), mask.has_value() ? mask->data_ptr() : nullptr, M, C, relu, cur());
@@ -53,9 +83,10 @@ void bn_apply(Tensor y, Tensor scale, Tensor shift, OptT res, OptT res_scale, Op
 }
 
 void channel_stats(Tensor y, Tensor sum, Tensor sqsum) {
-  chk(y, at::kBFloat16, "y");
-  const int C = (int)y.size(-1);
-  TORCH_CHECK(C % 8 == 0 && C <= 2048);
+  const int C = act_channels(y, "y");
+  TORCH_CHECK(C <= 2048, "channel_stats: at most 2048 channels");
+  vec(sum, at::kFloat, C, "sum", 1);
+  vec(sqsum, at::kFloat, C, "sqsum", 1);
   b200::channel_stats(y.data_ptr(), sum.data_ptr<float>(), sqsum.data_ptr<float>(), y.numel() / C, C, cur());
   after();
 }
@@ -63,13 +94,23 @@ void channel_stats(Tensor y, Tensor sum, Tensor sqsum) {
 // mode: 1 = ReLU mask from `outp` (g2 / dz_out optional), 2 = mask from y*scale+shift, 3 = no mask
 void bn_bwd_reduce(int64_t mode, Tensor g1, OptT g2, OptT outp, Tensor y, OptT scale, OptT shift, OptT dz_out,
                    Tensor sum_dz, Tensor sum_dzy) {
-  chk(g1, at::kBFloat16, "g1");
-  chk(y, at::kBFloat16, "y");
-  const int C = (int)y.size(-1);
-  TORCH_CHECK(C % 8 == 0 && C <= 2048 && g1.numel() == y.numel());
+  const int C = act_channels(y, "y");
+  TORCH_CHECK(C <= 2048, "bn_bwd_reduce: at most 2048 channels");
+  same_act(g1, y, "g1");
   TORCH_CHECK(mode >= 1 && mode <= 4);
   TORCH_CHECK((mode != 1 && mode != 4) || outp.has_value(), "modes 1/4 need the activation output / bitmask");
   TORCH_CHECK(mode != 2 || (scale.has_value() && shift.has_value()), "mode 2 needs scale/shift");
+  // operands a mode does not read must be absent, so that a call never silently ignores one
+  TORCH_CHECK(mode == 1 || mode == 4 || (!g2.has_value() && !outp.has_value() && !dz_out.has_value()),
+              "g2 / outp / dz_out are used by modes 1 and 4 only");
+  TORCH_CHECK(mode == 2 || (!scale.has_value() && !shift.has_value()), "scale / shift are used by mode 2 only");
+  if (g2.has_value()) same_act(*g2, y, "g2");
+  if (dz_out.has_value()) same_act(*dz_out, y, "dz_out");
+  if (mode == 1) same_act(*outp, y, "outp");
+  if (mode == 4) vec(*outp, at::kByte, y.numel() / 8, "outp (bitmask)", 1);
+  if (mode == 2) { vec(*scale, at::kFloat, C, "scale"); vec(*shift, at::kFloat, C, "shift"); }
+  vec(sum_dz, at::kFloat, C, "sum_dz", 1);
+  vec(sum_dzy, at::kFloat, C, "sum_dzy", 1);
   b200::bn_bwd_reduce((int)mode, g1.data_ptr(), vp(g2), vp(outp), y.data_ptr(), fp(scale), fp(shift),
                       dz_out.has_value() ? dz_out->data_ptr() : nullptr, sum_dz.data_ptr<float>(),
                       sum_dzy.data_ptr<float>(), y.numel() / C, C, cur());
@@ -79,6 +120,10 @@ void bn_bwd_reduce(int64_t mode, Tensor g1, OptT g2, OptT outp, Tensor y, OptT s
 void bn_bwd_coeffs(Tensor sum_dz, Tensor sum_dzy, Tensor gamma, Tensor mean, Tensor invstd, double count,
                    Tensor dgamma, Tensor dbeta, Tensor cA, Tensor cB, Tensor cC) {
   const int C = (int)gamma.numel();
+  for (const auto& [t, name] : {std::pair<const Tensor*, const char*>{&sum_dz, "sum_dz"}, {&sum_dzy, "sum_dzy"},
+                                {&gamma, "gamma"}, {&mean, "mean"}, {&invstd, "invstd"}, {&dgamma, "dgamma"},
+                                {&dbeta, "dbeta"}, {&cA, "cA"}, {&cB, "cB"}, {&cC, "cC"}})
+    vec(*t, at::kFloat, C, name, 1);
   b200::bn_bwd_coeffs(sum_dz.data_ptr<float>(), sum_dzy.data_ptr<float>(), gamma.data_ptr<float>(),
                       mean.data_ptr<float>(), invstd.data_ptr<float>(), count, dgamma.data_ptr<float>(),
                       dbeta.data_ptr<float>(), cA.data_ptr<float>(), cB.data_ptr<float>(), cC.data_ptr<float>(), C,
@@ -86,12 +131,21 @@ void bn_bwd_coeffs(Tensor sum_dz, Tensor sum_dzy, Tensor gamma, Tensor mean, Ten
   after();
 }
 
-// dy = A*dz + B*y + C;  dz = g (scale absent) or g * (y*scale+shift > 0)
+// dz = g, or g * (y*scale + shift > 0) when scale / shift are given: both or neither, C fp32 values each
+static void bn_bwd_apply_operands(const Tensor& g, const Tensor& y, const OptT& scale, const OptT& shift, const Tensor& dy,
+                                  int C) {
+  same_act(g, y, "g");
+  same_act(dy, y, "dy");
+  TORCH_CHECK(scale.has_value() == shift.has_value(), "scale and shift go together");
+  if (scale.has_value()) { vec(*scale, at::kFloat, C, "scale"); vec(*shift, at::kFloat, C, "shift"); }
+}
+
 void bn_bwd_apply(Tensor g, Tensor y, OptT scale, OptT shift, Tensor cA, Tensor cB, Tensor cC, Tensor dy) {
-  chk(g, at::kBFloat16, "g");
-  chk(y, at::kBFloat16, "y");
-  chk(dy, at::kBFloat16, "dy");
-  const int C = (int)y.size(-1);
+  const int C = act_channels(y, "y");
+  bn_bwd_apply_operands(g, y, scale, shift, dy, C);
+  vec(cA, at::kFloat, C, "cA");
+  vec(cB, at::kFloat, C, "cB");
+  vec(cC, at::kFloat, C, "cC");
   b200::bn_bwd_apply(g.data_ptr(), y.data_ptr(), fp(scale), fp(shift), cA.data_ptr<float>(), cB.data_ptr<float>(),
                      cC.data_ptr<float>(), dy.data_ptr(), y.numel() / C, C, cur());
   after();
@@ -123,12 +177,11 @@ static b200::BnFwdFuse fwd_fuse(const Tensor& sum, const Tensor& sqsum, const Te
 // pack order (main BN and `res_pack`): sum, sqsum, gamma, beta, running_mean, running_var, mean, invstd, scale, shift
 void bn_apply_fused(Tensor y, std::vector<Tensor> pack, double count, double momentum, double eps, OptT res,
                     c10::optional<std::vector<Tensor>> res_pack, Tensor out, bool relu, OptT mask) {
-  chk(y, at::kBFloat16, "y");
-  chk(out, at::kBFloat16, "out");
-  const int C = (int)y.size(-1);
+  const int C = act_channels(y, "y");
   const int64_t M = y.numel() / C;
-  TORCH_CHECK(C % 8 == 0 && out.numel() == y.numel() && pack.size() == 10);
-  if (res.has_value()) { chk(*res, at::kBFloat16, "res"); TORCH_CHECK(res->numel() == y.numel()); }
+  same_act(out, y, "out");
+  TORCH_CHECK(pack.size() == 10);
+  if (res.has_value()) same_act(*res, y, "res");
   if (mask.has_value()) { chk(*mask, at::kByte, "mask"); TORCH_CHECK(mask->numel() * 8 == y.numel()); }
   TORCH_CHECK(!res_pack.has_value() || res.has_value(), "res_pack needs res");
   b200::BnFwdFuse f = fwd_fuse(pack[0], pack[1], pack[2], pack[3], pack[4], pack[5], pack[6], pack[7], pack[8], pack[9],
@@ -147,10 +200,8 @@ void bn_apply_fused(Tensor y, std::vector<Tensor> pack, double count, double mom
 // dy = A*dz + B*y + C with A, B, C computed in the kernel from sum_dz, sum_dzy; dgamma / dbeta written by the kernel.
 void bn_bwd_apply_fused(Tensor g, Tensor y, OptT scale, OptT shift, Tensor sum_dz, Tensor sum_dzy, Tensor gamma,
                         Tensor mean, Tensor invstd, double count, Tensor dgamma, Tensor dbeta, Tensor dy) {
-  chk(g, at::kBFloat16, "g");
-  chk(y, at::kBFloat16, "y");
-  chk(dy, at::kBFloat16, "dy");
-  const int C = (int)y.size(-1);
+  const int C = act_channels(y, "y");
+  bn_bwd_apply_operands(g, y, scale, shift, dy, C);
   for (const Tensor* t : {&sum_dz, &sum_dzy, &gamma, &mean, &invstd, &dgamma, &dbeta}) {
     TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->numel() == C && t->is_contiguous());
     TORCH_CHECK(reinterpret_cast<uintptr_t>(t->data_ptr()) % 16 == 0, "fused BN parameter must be 16-byte aligned");
@@ -164,44 +215,59 @@ void bn_bwd_apply_fused(Tensor g, Tensor y, OptT scale, OptT shift, Tensor sum_d
   after();
 }
 
+// 3x3/2 pad-1 max pool: x bf16 NHWC [N, H, W, C], pooled [N, Ho, Wo, C] bf16 and its uint8 argmax of the same shape
+static void pool_shapes(const Tensor& x, const Tensor& pooled, const char* pname, const OptT& idx) {
+  TORCH_CHECK(x.dim() == 4, "max pool: NHWC input");
+  const int C = act_channels(x, "pool input");
+  chk(pooled, at::kBFloat16, pname);
+  aligned(pooled, 16, pname);
+  const int64_t Ho = (x.size(1) - 1) / 2 + 1, Wo = (x.size(2) - 1) / 2 + 1;
+  TORCH_CHECK(pooled.dim() == 4 && pooled.size(0) == x.size(0) && pooled.size(1) == Ho && pooled.size(2) == Wo &&
+              pooled.size(3) == C, pname, " must be [N, (H+1)/2, (W+1)/2, C]");
+  if (idx.has_value()) vec(*idx, at::kByte, pooled.numel(), "idx", 8);
+}
+
 void maxpool_fwd(Tensor x, Tensor out, OptT idx) {
-  chk(x, at::kBFloat16, "x");
-  chk(out, at::kBFloat16, "out");
-  if (idx.has_value()) { chk(*idx, at::kByte, "idx"); TORCH_CHECK(idx->numel() == out.numel()); }
+  pool_shapes(x, out, "out", idx);
   b200::maxpool_fwd(x.data_ptr(), out.data_ptr(), idx.has_value() ? idx->data_ptr() : nullptr, (int)x.size(0),
                     (int)x.size(1), (int)x.size(2), (int)x.size(3), cur());
   after();
 }
 void bn_relu_maxpool_fwd(Tensor y, Tensor scale, Tensor shift, Tensor out, OptT idx) {
-  chk(y, at::kBFloat16, "y");
-  chk(out, at::kBFloat16, "out");
-  chk(scale, at::kFloat, "scale");
-  chk(shift, at::kFloat, "shift");
-  if (idx.has_value()) { chk(*idx, at::kByte, "idx"); TORCH_CHECK(idx->numel() == out.numel()); }
+  pool_shapes(y, out, "out", idx);
+  vec(scale, at::kFloat, y.size(3), "scale");
+  vec(shift, at::kFloat, y.size(3), "shift");
   b200::bn_relu_maxpool_fwd(y.data_ptr(), scale.data_ptr<float>(), shift.data_ptr<float>(), out.data_ptr(),
                             idx.has_value() ? idx->data_ptr() : nullptr, (int)y.size(0), (int)y.size(1),
                             (int)y.size(2), (int)y.size(3), cur());
   after();
 }
 void maxpool_bwd(Tensor idx, Tensor g1, OptT g2, Tensor dx) {
-  chk(idx, at::kByte, "idx");
-  chk(g1, at::kBFloat16, "g1");
-  chk(dx, at::kBFloat16, "dx");
+  pool_shapes(dx, g1, "g1", idx);
+  if (g2.has_value()) same_act(*g2, g1, "g2");
   b200::maxpool_bwd(idx.data_ptr(), g1.data_ptr(), vp(g2), dx.data_ptr(), (int)dx.size(0), (int)dx.size(1),
                     (int)dx.size(2), (int)dx.size(3), cur());
   after();
 }
+// global average pool: x bf16 [N, ..., C] (HW = the middle extent), pooled bf16 [N, C]
+static int gap_shapes(const Tensor& x, const Tensor& pooled, double drop_p) {
+  TORCH_CHECK(x.dim() >= 2 && x.size(0) > 0, "global average pool: [N, ..., C] input");
+  const int C = act_channels(x, "pool input");
+  TORCH_CHECK(x.numel() / x.size(0) / C > 0, "global average pool: empty spatial extent");
+  chk(pooled, at::kBFloat16, "pooled");
+  aligned(pooled, 16, "pooled");
+  TORCH_CHECK(pooled.numel() == x.size(0) * C, "pooled must have N * C elements");
+  TORCH_CHECK(drop_p >= 0.0 && drop_p < 1.0, "dropout probability must be in [0, 1)");
+  return C;
+}
+
 void gap_fwd(Tensor x, Tensor out, double drop_p, int64_t seed) {
-  chk(x, at::kBFloat16, "x");
-  chk(out, at::kBFloat16, "out");
-  const int N = (int)x.size(0), C = (int)x.size(-1);
+  const int N = (int)x.size(0), C = gap_shapes(x, out, drop_p);
   b200::gap_fwd(x.data_ptr(), out.data_ptr(), N, (int)(x.numel() / N / C), C, (float)drop_p, (uint64_t)seed, cur());
   after();
 }
 void gap_bwd(Tensor dout, Tensor dx, double drop_p, int64_t seed) {
-  chk(dout, at::kBFloat16, "dout");
-  chk(dx, at::kBFloat16, "dx");
-  const int N = (int)dx.size(0), C = (int)dx.size(-1);
+  const int N = (int)dx.size(0), C = gap_shapes(dx, dout, drop_p);
   b200::gap_bwd(dout.data_ptr(), dx.data_ptr(), N, (int)(dx.numel() / N / C), C, (float)drop_p, (uint64_t)seed, cur());
   after();
 }
@@ -262,7 +328,11 @@ void stem_pool_bn_bwd(int64_t pass, Tensor idx, Tensor g1, OptT g2, Tensor y, Te
   TORCH_CHECK(Ho % 8 == 0 && Wo % 8 == 0, "stem tail: pooled grid must tile by 8");
   if (g2.has_value()) { chk(*g2, at::kBFloat16, "g2"); TORCH_CHECK(g2->numel() == g1.numel()); }
   TORCH_CHECK(pass == 0 || (cA.has_value() && cB.has_value() && cC.has_value() && dy.has_value()));
-  if (dy.has_value()) { chk(*dy, at::kBFloat16, "dy"); TORCH_CHECK(dy->numel() == y.numel()); }
+  if (dy.has_value()) same_act(*dy, y, "dy");
+  aligned(y, 16, "y");
+  for (const auto& [t, name] : {std::pair<const OptT, const char*>{scale, "scale"}, {shift, "shift"}, {cA, "cA"}, {cB, "cB"},
+                                {cC, "cC"}, {sum_dz, "sum_dz"}, {sum_dzy, "sum_dzy"}})
+    if (t.has_value()) vec(*t, at::kFloat, 64, name, 1);
   b200::stem_pool_bn_bwd((int)pass, idx.data_ptr(), g1.data_ptr(), vp(g2), y.data_ptr(), scale.data_ptr<float>(),
                          shift.data_ptr<float>(), fp(cA), fp(cB), fp(cC), dy.has_value() ? dy->data_ptr() : nullptr,
                          sum_dz.data_ptr<float>(), sum_dzy.data_ptr<float>(), N, Ho, Wo, cur());
@@ -284,6 +354,7 @@ void mbv2_stem(Tensor x, Tensor w, Tensor scale, Tensor shift, Tensor out, doubl
   TORCH_CHECK(w.numel() == 27 * 32 && scale.numel() >= 32 && shift.numel() >= 32);
   TORCH_CHECK(out.dim() == 4 && out.size(0) == x.size(0) && out.size(1) == x.size(1) / 2 && out.size(2) == x.size(2) / 2 &&
               out.size(3) >= 32 && out.size(3) % 8 == 0);
+  aligned(out, 16, "out");
   b200::mbv2_stem(x.data_ptr<uint8_t>(), w.data_ptr<float>(), scale.data_ptr<float>(), shift.data_ptr<float>(), out.data_ptr(),
                   (int)x.size(0), (int)x.size(1), (int)x.size(2), (int)out.size(3), (float)mul, (float)add, cur());
   after();
@@ -300,6 +371,7 @@ void dwconv3x3(Tensor x, Tensor w, Tensor scale, Tensor shift, Tensor out, int64
   TORCH_CHECK(x.dim() == 4 && C % 8 == 0 && w.numel() == 9 * C && scale.numel() == C && shift.numel() == C);
   TORCH_CHECK(out.dim() == 4 && out.size(0) == x.size(0) && out.size(3) == C && out.size(1) == (H - 1) / stride + 1 &&
               out.size(2) == (W - 1) / stride + 1, "dwconv3x3 output shape");
+  for (const Tensor* t : {&x, &w, &scale, &shift, &out}) aligned(*t, 16, "dwconv3x3 operand");
   b200::dwconv3x3(x.data_ptr(), w.data_ptr<float>(), scale.data_ptr<float>(), shift.data_ptr<float>(), out.data_ptr(),
                   (int)x.size(0), H, W, C, (int)stride, (int)tile_w, cur());
   after();
@@ -325,6 +397,8 @@ void resize_bilinear_u8(Tensor x, Tensor out, bool planar) {
 void weight_prep(Tensor w, OptT wf, OptT wd, int64_t taps, int64_t cout, int64_t cin) {
   chk(w, at::kFloat, "w");
   TORCH_CHECK(w.numel() == taps * cout * cin);
+  if (wf.has_value()) vec(*wf, at::kBFloat16, w.numel(), "wf", 1);
+  if (wd.has_value()) vec(*wd, at::kBFloat16, w.numel(), "wd", 1);
   b200::weight_prep(w.data_ptr<float>(), wf.has_value() ? wf->data_ptr() : nullptr,
                     wd.has_value() ? wd->data_ptr() : nullptr, (int)taps, (int)cout, (int)cin, cur());
   after();
@@ -339,30 +413,41 @@ void weight_prep_batched(Tensor params, Tensor wd, Tensor table, int64_t total) 
                             total, cur());
   after();
 }
+// flat fp32 buffers read as float4, the bf16 working copy written 4 values (8 bytes) at a time
+static void optim_operands(const Tensor& p, std::initializer_list<std::pair<const Tensor*, const char*>> state,
+                           const OptT& p16, const Tensor& hyper) {
+  chk(p, at::kFloat, "p");
+  TORCH_CHECK(p.numel() % 4 == 0, "p: element count must be a multiple of 4");
+  aligned(p, 16, "p");
+  for (const auto& [t, name] : state) vec(*t, at::kFloat, p.numel(), name);
+  if (p16.has_value()) vec(*p16, at::kBFloat16, p.numel(), "p16", 8);
+  vec(hyper, at::kFloat, hyper.numel(), "hyper", 1);
+  TORCH_CHECK(hyper.numel() >= b200::kHyperLen, "hyper must hold 8 values");
+}
+
 void sgd_step(Tensor p, Tensor g, Tensor mom, OptT p16, Tensor hyper, bool nesterov) {
-  chk(p, at::kFloat, "p"); chk(g, at::kFloat, "g"); chk(mom, at::kFloat, "mom"); chk(hyper, at::kFloat, "hyper");
-  TORCH_CHECK(p.numel() % 4 == 0 && g.numel() == p.numel() && mom.numel() == p.numel() && hyper.numel() >= b200::kHyperLen);
+  optim_operands(p, {{&g, "g"}, {&mom, "mom"}}, p16, hyper);
   b200::sgd_step(p.data_ptr<float>(), g.data_ptr<float>(), mom.data_ptr<float>(),
                  p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), nesterov, cur());
   after();
 }
 void adam_step(Tensor p, Tensor g, Tensor m, Tensor v, OptT p16, Tensor hyper) {
-  chk(p, at::kFloat, "p"); chk(g, at::kFloat, "g"); chk(m, at::kFloat, "m"); chk(v, at::kFloat, "v");
-  TORCH_CHECK(p.numel() % 4 == 0 && g.numel() == p.numel() && hyper.numel() >= b200::kHyperLen);
+  optim_operands(p, {{&g, "g"}, {&m, "m"}, {&v, "v"}}, p16, hyper);
   b200::adam_step(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
                   p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
   after();
 }
 void adadelta_step(Tensor p, Tensor g, Tensor sq, Tensor acc, OptT p16, Tensor hyper) {
-  chk(p, at::kFloat, "p"); chk(g, at::kFloat, "g");
-  TORCH_CHECK(p.numel() % 4 == 0 && g.numel() == p.numel() && hyper.numel() >= b200::kHyperLen);
+  optim_operands(p, {{&g, "g"}, {&sq, "sq"}, {&acc, "acc"}}, p16, hyper);
   b200::adadelta_step(p.data_ptr<float>(), g.data_ptr<float>(), sq.data_ptr<float>(), acc.data_ptr<float>(),
                       p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
   after();
 }
 void cast_bf16(Tensor x, Tensor out) {
-  chk(x, at::kFloat, "x"); chk(out, at::kBFloat16, "out");
-  TORCH_CHECK(x.numel() % 4 == 0 && out.numel() == x.numel());
+  chk(x, at::kFloat, "x");
+  TORCH_CHECK(x.numel() % 4 == 0, "x: element count must be a multiple of 4");
+  aligned(x, 16, "x");
+  vec(out, at::kBFloat16, x.numel(), "out", 8);
   b200::cast_f32_to_bf16(x.data_ptr<float>(), out.data_ptr(), x.numel(), cur());
   after();
 }

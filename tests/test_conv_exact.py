@@ -22,16 +22,14 @@ every dispatch branch of ``conv_igemm.cu``, each at one tile per CTA and at seve
 """
 from __future__ import annotations
 
-import math
 from dataclasses import dataclass
 
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from exact_util import DEV, Guarded, check_equal, check_sum, pack_mask, tern, to_bf16_exact
 
-DEV = "cuda"
-U = 2.0 ** -24   # fp32 unit round-off
+pytestmark = pytest.mark.gpu
 
 
 def _C():
@@ -45,87 +43,6 @@ def _ops():
     from b200ddl import ops
 
     return ops.ext("_b200_ops")
-
-
-# ----------------------------------------------------------------------------------------------------------- data
-def tern(shape, gen, density=0.6, hi=1):
-    """fp32 tensor of {-1, 0, 1}; with ``hi > 1`` a quarter of the non-zeros are +-hi instead."""
-    v = (torch.randint(0, 2, shape, device=DEV, generator=gen) * 2 - 1).float()
-    v *= (torch.rand(shape, device=DEV, generator=gen) < density).float()
-    if hi > 1:
-        v *= torch.where(torch.rand(shape, device=DEV, generator=gen) < 0.25, float(hi), 1.0)
-    return v
-
-
-class Guarded:
-    """``t``: a tensor of ``shape`` inside a larger allocation whose ``guard`` elements before and after it are NaN."""
-
-    def __init__(self, shape, dtype, fill, guard=4096):
-        n = math.prod(shape)
-        self.guard = guard
-        self.buf = torch.full((n + 2 * guard,), float("nan"), dtype=dtype, device=DEV)
-        self.t = self.buf[guard:guard + n].view(shape)
-        self.t.fill_(fill)
-        self._bits = self._as_int(self.buf).clone()
-
-    @staticmethod
-    def _as_int(t):
-        return t.view(torch.int16 if t.element_size() == 2 else torch.int32)
-
-    def check_guards(self, name):
-        b = self._as_int(self.buf)
-        g = self.guard
-        for side, a, ref in (("before", b[:g], self._bits[:g]), ("after", b[-g:], self._bits[-g:])):
-            bad = (a != ref).nonzero().flatten()
-            if bad.numel():
-                pytest.fail(f"{name}: {bad.numel()} guard elements {side} the output were written (first at offset "
-                            f"{int(bad[0]) - (g if side == 'before' else 0)})")
-
-
-def check_equal(name, out, exp, locate=None):
-    """Exact comparison (NaN, i.e. an element never written, is a mismatch); reports the first mismatches with their
-    kernel tile coordinates."""
-    o, e = out.double(), exp.double()
-    bad = ~(o == e)
-    n = int(bad.sum())
-    if n == 0:
-        return
-    lines = []
-    for ix in bad.nonzero()[:8].tolist():
-        where = locate(*ix) if locate is not None else ""
-        lines.append(f"  at {tuple(ix)}: got {o[tuple(ix)].item()} want {e[tuple(ix)].item()} {where}")
-    pytest.fail(f"{name}: {n} of {o.numel()} elements differ\n" + "\n".join(lines))
-
-
-def check_sum(name, got, ref, ref_abs, depth):
-    """Per-channel fp32 sums of integer terms.  ``ref_abs`` = sum of |terms| (float64).  Below 2^24 every partial sum,
-    in any order, is an integer that fp32 holds exactly: equality is demanded.  Above, each fp32 addition on a term's
-    path to the result errs by at most u * |partial| <= u * sum|terms|, and no term passes more than ``depth`` additions,
-    so |error| <= depth * u * sum|terms| (first order in u)."""
-    got = got.double()
-    if float(ref_abs.max()) < 2.0 ** 24:
-        check_equal(name, got, ref)
-        return "exact"
-    bound = depth * U * ref_abs * (1 + 1e-6)
-    err = (got - ref).abs()
-    if not bool((err <= bound).all()):
-        c = int((err - bound).argmax())
-        pytest.fail(f"{name}: channel {c} got {got[c].item()} want {ref[c].item()} (error {err[c].item():.3e} > bound "
-                    f"{bound[c].item():.3e}, sum|terms| {ref_abs[c].item():.3e}, depth {depth})")
-    return "bounded"
-
-
-def to_bf16_exact(ref):
-    """bf16 of a float64 tensor holding values exact in fp32 (round to nearest even, like __floats2bfloat162_rn)."""
-    assert bool((ref.float().double() == ref).all()), "reference is not exact in fp32"
-    return ref.float().to(torch.bfloat16)
-
-
-def pack_mask(mask_bool):
-    """[M, C] bool -> uint8 [M * C / 8]; bit k of byte j = channel 8 j + k (the layout bn_apply writes)."""
-    M, C_ = mask_bool.shape
-    bits = mask_bool.view(M, C_ // 8, 8).to(torch.int32)
-    return (bits * (2 ** torch.arange(8, device=DEV, dtype=torch.int32))).sum(-1).to(torch.uint8).view(-1).contiguous()
 
 
 def nchw(t):
