@@ -113,8 +113,9 @@ struct ConvPlan {
     }
     // Tile width: the wider N tile re-reads the A operand less, but a persistent grid of one CTA per SM pays for whole
     // waves.  The cost model is waves x tile width (the MMA time of a tile is proportional to its width); the narrower
-    // tile is taken only when it wins by >= 10 %.  128 is the widest: the two consumer warpgroups hold a 64 x BLOCK_N fp32
-    // accumulator each in registers.  B200DDL_BLOCK_N=128|64 forces a width (A/B measurements).
+    // tile is taken only when it wins by >= 10 %.  128 is the widest: each consumer warpgroup holds a whole tile's
+    // 128 x BLOCK_N fp32 accumulator in registers (128 per thread at BLOCK_N = 128).  B200DDL_BLOCK_N=128|64 forces a
+    // width (A/B measurements).
     {
       const int cap_ = max_ctas > 0 ? (int)max_ctas : sm_count();
       auto cost = [&](int bn) {
@@ -176,6 +177,8 @@ struct ConvPlan {
       TORCH_CHECK(bwd_y->sizes() == out.sizes() && bwd_y->is_contiguous(), "bwd_y must match the (dense) output");
       TORCH_CHECK(relu_mask->is_cuda() && relu_mask->scalar_type() == at::kByte && relu_mask->is_contiguous() &&
                       relu_mask->numel() == N * Ho * Wo * cout / 8, "relu_mask must be uint8 [M * Cout / 8]");
+      // the epilogue reads the mask bits of 64 channels as one 8-byte word
+      TORCH_CHECK(reinterpret_cast<uintptr_t>(relu_mask->data_ptr()) % 8 == 0, "relu_mask must be 8-byte aligned");
       TORCH_CHECK(add_src.has_value(), "the block-gradient epilogue needs the skip gradient");
       check_nhwc_view(*add_src, "add_src");
       TORCH_CHECK(add_src->is_contiguous() && add_src->size(0) == N && add_src->size(3) == cout, "add_src: dense NHWC with Cout channels");

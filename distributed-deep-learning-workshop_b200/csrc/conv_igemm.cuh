@@ -8,14 +8,18 @@
 //   out-of-bounds fill, so there is no im2col buffer.  Strided convs pass up to 4 "parity" views of the input (each a
 //   strided NHWC view) and a tap table that says which view + offset each tap reads.
 // * B is the filter as a [taps*Cout, Cin] K-major matrix.
-// * Warp-specialised, persistent: warp 8 = TMA producer (ONE thread chosen with elect.sync, integer smem addresses),
-//   warps 0-7 = two consumer warpgroups.  Warpgroup g owns rows 64g .. 64g+63 of the 128-row tile: it issues
-//   wgmma.m64nBLOCK_Nk16 from the shared-memory stages (accumulators in registers), then runs the epilogue itself
-//   (bf16 -> swizzled smem -> TMA store).  While the consumers run the epilogue of tile i the producer already fills
-//   the stage ring for tile i+1.
-// * kStats = 1: after staging each 64-column chunk the consumers reduce per-channel sum / sum-of-squares of the staged
-//   bf16 tile (register accumulators across tiles, one global atomic per channel and row group per CTA) - no separate
-//   BatchNorm statistics pass (SURVEY.md K10).
+// * Warp-specialised, persistent: warp 8 = TMA producer (ONE thread chosen with elect.sync, integer smem addresses;
+//   warps 9-11 only complete its warpgroup so that setmaxnreg can move registers to the consumers),
+//   warps 0-7 = two consumer warpgroups in ping-pong.  Warpgroup g owns the CTA's tiles g, g + 2, g + 4, ... whole: it
+//   issues two wgmma.m64nBLOCK_Nk16 per k-step (A rows 0 and 64 of the stage, 128 x BLOCK_N fp32 accumulators in
+//   registers), then runs the epilogue of that tile itself (bf16 -> its own swizzled staging buffers -> TMA store).
+//   The epilogue of tile i overlaps the main loop of tile i+1 on the other warpgroup.  An ordering barrier hands the
+//   main loop from one warpgroup to the other once all of a tile's MMAs are issued: the tensor cores see the tiles in
+//   CTA order, and a warpgroup never waits on a stage of the ring more than one lap ahead of the producer (with tiles
+//   of >= kStages stages that parity wait would pass on the previous lap's phase).
+// * kStats = 1: after staging each 64-column chunk the warpgroup reduces per-channel sum / sum-of-squares of its staged
+//   bf16 tile (register accumulators across its tiles, one global atomic per channel and 32-row group whenever its next
+//   tile moves to another n-block) - no separate BatchNorm statistics pass (SURVEY.md K10).
 //   kStats = 2: the same reduction for the BatchNorm-BACKWARD inside a dgrad GEMM (sum dz, sum dz*y with
 //   dz = g * [y*scale + shift > 0]; the pre-BN tile y arrives by an extra TMA load).
 // * kResB: the CTA's whole filter slice (<= 9 tiles of 8 KB, single N-block of 64 channels) stays resident in shared
@@ -49,22 +53,28 @@ constexpr int kResBBytes = 9 * 64 * kBlockK * 2;  // 72 KB = nine [64 x 64] bf16
 
 constexpr int kHaloRows = 224;  // largest halo box: bw * (bh + 2) pixels (56 x 4); 28 KB per stage
 
-constexpr int kConvConsumers = 256;               // two warpgroups
-constexpr int kConvThreads = kConvConsumers + 32;  // + the producer warp
+constexpr int kConvConsumers = 256;                // two warpgroups
+constexpr int kConvThreads = kConvConsumers + 128;  // + the producer warpgroup (one working warp)
+// Register split (setmaxnreg): the kernel launches at 65536 / 384 -> 168 registers per thread; the producer warpgroup
+// drops to 40 and the consumers rise to 232, room for a whole tile's 128 fp32 accumulators at BLOCK_N = 128.
+// 128 * 40 + 256 * 232 = 64512 <= 65536.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 constexpr int kSmemLimit = 232448;                 // 227 KB per block
 constexpr int kAlignSlack = 1024;                  // dynamic smem is rounded up to 1024 B in the kernel
+constexpr int kTileChunkBytes = kBlockM * 128;     // one 128 x 64 bf16 tile chunk (16 KB)
 
 template <int BLOCK_N, int kStats = 0, bool kResB = false, bool kHalo = false>
 struct ConvSmem {
-  // Two pre-BN tile buffers, loaded at the start of their own chunk.
-  static constexpr int kYBufs = 2;
-  static constexpr int kYBytes = (kStats == 2 || kStats == 3) ? kYBufs * kBlockM * 128 : 0;  // 128x64 bf16 tiles of y
+  // Per warpgroup: one pre-BN tile buffer (loaded at the start of its own chunk) and one store buffer per 64-column
+  // chunk of the tile, so neither warpgroup's stores or loads wait for the other's.
+  static constexpr int kYBytes = (kStats == 2 || kStats == 3) ? 2 * kTileChunkBytes : 0;  // 128x64 bf16 tiles of y
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kASlot = kHalo ? kHaloRows * 128 : kABytes;     // bytes of A per pipeline stage
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = kResB ? kASlot : kASlot + kBBytes;
   static constexpr int kResBytes = kResB ? kResBBytes : 0;
-  static constexpr int kStagingBytes = 2 * kBlockM * 128;  // two 128x64 bf16 store buffers
+  static constexpr int kStagingBytes = 2 * (BLOCK_N / 64) * kTileChunkBytes;  // per warpgroup: BLOCK_N / 64 buffers
   static constexpr int kBarBytes = 256;
   static constexpr int kFixed = kResBytes + kStagingBytes + kYBytes + kBarBytes + 16;
   static constexpr int kFit = (kSmemLimit - kAlignSlack - kFixed) / kStageBytes;  // stages that fit beside the fixed buffers
@@ -79,14 +89,19 @@ struct ConvSmem {
 };
 
 // Four K-steps of 16 (one 64-wide k-block, one 128 B swizzle row): +32 B = +2 in the descriptor's address field each.
+// Each K-step runs twice, for A rows 0..63 into acc[0] and rows 64..127 (8 KB further: +512, whole swizzle atoms) into
+// acc[1].
 template <int BLOCK_N>
-__device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint64_t da, uint64_t db) {
+__device__ __forceinline__ void mma_kblock(float (&acc)[2][BLOCK_N / 2], uint64_t da, uint64_t db) {
 #pragma unroll
   for (int k = 0; k < kBlockK / 16; ++k) {
-    if constexpr (BLOCK_N == 128)
-      wgmma_m64n128k16<0, 0>(acc, da + 2 * k, db + 2 * k);
-    else
-      wgmma_m64n64k16<0, 0>(acc, da + 2 * k, db + 2 * k);
+#pragma unroll
+    for (int mh = 0; mh < 2; ++mh) {
+      if constexpr (BLOCK_N == 128)
+        wgmma_m64n128k16<0, 0>(acc[mh], da + mh * 512 + 2 * k, db + 2 * k);
+      else
+        wgmma_m64n64k16<0, 0>(acc[mh], da + mh * 512 + 2 * k, db + 2 * k);
+    }
   }
 }
 
@@ -101,7 +116,7 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
   constexpr bool kHasY = kStats == 2 || kStats == 3;     // a pre-BN tile accompanies every output chunk
   constexpr bool kAffine = kStats == 4;                  // epilogue: acc*scale + shift (+ residual) -> activation
   constexpr int kChunks = BLOCK_N / 64;
-  constexpr int kAcc = BLOCK_N / 2;                      // fp32 accumulators per consumer thread
+  constexpr int kAcc = BLOCK_N / 2;                      // fp32 accumulators per thread and 64-row half of the tile
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
@@ -112,7 +127,7 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(sY + L::kYBytes);
   uint64_t* full_bar = bars;                     // [kStages]
   uint64_t* empty_bar = bars + kStages;          // [kStages]
-  uint64_t* y_bar = bars + 2 * kStages;          // [2] (kHasY)
+  uint64_t* y_bar = bars + 2 * kStages;          // [2] (kHasY): one per warpgroup
   uint64_t* bres_bar = bars + 2 * kStages + 2;   // resident filter loaded (kResB)
   int* s_last = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(bars) + L::kBarBytes);
 
@@ -127,7 +142,7 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
     tma_prefetch_desc(&tmD);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kConvConsumers / 32);  // one arrival per consumer warp
+      mbar_init(&empty_bar[i], 4);  // one arrival per warp of the warpgroup that consumed the stage
     }
     for (int i = 0; i < 2; ++i) mbar_init(&y_bar[i], 1);
     mbar_init(bres_bar, 1);
@@ -144,8 +159,9 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
   const uint32_t a_bytes = (p.mode == 0 ? kBlockM : p.valid_rows) * 128;
   const uint32_t stage_tx = kHalo ? static_cast<uint32_t>(p.halo_bytes) : (kResB ? a_bytes : a_bytes + L::kBBytes);
 
-  if (warp == kConvConsumers / 32) {
-    if (elect_one()) {
+  if (warp >= kConvConsumers / 32) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kConvConsumers / 32 && elect_one()) {
       // ---------------------------------------------------------------- TMA producer (one elected thread)
       const int taps = p.taps, kblocks = p.kblocks, n_blocks = p.n_blocks, num_tiles = p.num_tiles, cout = p.cout;
       const bool flat = p.mode == 0;
@@ -220,17 +236,23 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
   }
 
   // -------------------------------------------------------------------- consumers: two warpgroups (256 threads)
+  setmaxnreg_inc<kConsumerRegs>();
   const int ctid = threadIdx.x;
-  const int wg = warp >> 2;                                  // rows 64*wg .. 64*wg+63 of the tile
-  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // accumulator rows of this thread: row0, row0 + 8
-  const int cq = (lane & 3) * 2;                             // column pair inside each 8-column group
-  const uint32_t full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
+  const int wg = warp >> 2;                       // warpgroup: the CTA's tiles wg, wg + 2, wg + 4, ...
+  const int wtid = ctid & 127;                    // thread in the warpgroup
+  const int r16 = (warp & 3) * 16 + (lane >> 2);  // accumulator rows of this thread: r16 + 8h + 64mh (h, mh in {0, 1})
+  const int cq = (lane & 3) * 2;                  // column pair inside each 8-column group
+  const uint32_t full0 = smem_u32(full_bar);
+  // named barriers: 1 + wg = this warpgroup's epilogue, 3 + wg = "warpgroup wg may start its next main loop"
+  // (bar.arrive by the other warpgroup + bar.sync by this one), 5 = both warpgroups before the last-CTA tail
+  const uint32_t epi_bar = 1 + wg, my_turn = 3 + wg, their_turn = 4 - wg;
   // descriptors differ only in the 14-bit start-address field (addr >> 4): build once, add per stage / k-step.
-  // The warpgroup's 64-row slice starts 8 KB into the A tile (a whole number of swizzle atoms).
-  const uint64_t da0 = gmma_desc_sw128(smem_u32(sA) + wg * 64 * 128, 16, 1024);
+  const uint64_t da0 = gmma_desc_sw128(smem_u32(sA), 16, 1024);
   const uint64_t db0 = gmma_desc_sw128(smem_u32(sB), 16, 1024);
-  // statistics: this thread reduces column pair cp of each staged chunk over the 16 rows of row group rg
-  const int cp = ctid & 31, rg = ctid >> 5;
+  uint8_t* const sStageW = sStage + wg * (kChunks * kTileChunkBytes);  // this warpgroup's store buffers, one per chunk
+  uint8_t* const sYW = sY + wg * kTileChunkBytes;                      // and its pre-BN tile buffer (kHasY)
+  // statistics: this thread reduces column pair cp of each staged chunk over the 32 rows of row group rg
+  const int cp = wtid & 31, rg = wtid >> 5;
   uint32_t xoff[8];  // byte offset of column pair cp in a row with (row & 7) == j
 #pragma unroll
   for (int j = 0; j < 8; ++j) xoff[j] = (((cp >> 2) ^ j) << 4) + ((cp & 3) << 2);
@@ -238,12 +260,13 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
 #pragma unroll
   for (int c = 0; c < kChunks; ++c) sacc[c][0] = sacc[c][1] = sacc[c][2] = sacc[c][3] = 0.f;
 
-  int stage = 0;
-  uint32_t phase = 0;
+  // Stages are consumed in CTA tile order, n_stages per tile: local tile i starts at ring position i * n_stages.
+  const int n_stages = kHalo ? 3 * p.kblocks : k_iters;
+  int ring = wg * n_stages;
   int chunk_ctr = 0;
   if (kResB && static_cast<int>(blockIdx.x) < p.num_tiles) mbar_wait(bres_bar, 0);
 
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+  for (int tile = blockIdx.x + wg * gridDim.x, i = wg; tile < p.num_tiles; tile += 2 * gridDim.x, i += 2) {
     const int m_tile = tile / p.n_blocks;
     const int nb = tile - m_tile * p.n_blocks;
     int w0 = 0, h0 = 0, n0 = 0;
@@ -255,16 +278,48 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
       h0 = th * p.bh;
       n0 = (rest / p.tiles_h) * p.bn;
     }
+    int stage = ring % kStages;
+    uint32_t phase = (ring / kStages) & 1;
+    ring += 2 * n_stages;
 
+    // kStats == 3 / kAffine residual: this thread's four rows of the additive tensor (flat mode: tile row == pixel
+    // index), row r16 + 8 * (q & 1) + 64 * (q >> 1) for q = 2 * mh + h.  Computed before the main loop (scalar work
+    // the MMAs hide); the loads themselves sit in the epilogue, under the other warpgroup's MMAs.
+    const __nv_bfloat16* arow[4] = {nullptr, nullptr, nullptr, nullptr};
+    const uint8_t* mrow[4] = {nullptr, nullptr, nullptr, nullptr};
+    if ((kStats == 3 || kAffine) && p.mode == 0 && (kStats == 3 || p.add_src != nullptr)) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int64_t grow = static_cast<int64_t>(m_tile) * kBlockM + r16 + 8 * (q & 1) + 64 * (q >> 1);
+        if (grow < p.m_rows) {
+          if (kStats == 3) mrow[q] = p.relu_mask + grow * (p.cout >> 3) + ((nb * BLOCK_N) >> 3);
+          if (p.add_mode == 0) {
+            arow[q] = p.add_src + grow * p.cout + nb * BLOCK_N;
+          } else {
+            // compact skip gradient of a stride-2 1x1 projection: only even (h, w) positions carry a value
+            const int wq = static_cast<int>(grow % p.add_w);
+            const int64_t t = grow / p.add_w;
+            const int hq = static_cast<int>(t % p.add_h);
+            const int64_t nq = t / p.add_h;
+            if (((wq | hq) & 1) == 0)
+              arow[q] = p.add_src + ((nq * (p.add_h >> 1) + (hq >> 1)) * (p.add_w >> 1) + (wq >> 1)) * p.cout + nb * BLOCK_N;
+          }
+        }
+      }
+    }
     // ---------------------------------------------------------------- main loop
     // One stage = one k-block (or, in halo mode, three vertical taps of one k-block).  The MMAs of a stage stay in
     // flight while the next stage is waited for; a stage is released once the group after it has been issued.
-    float acc[kAcc];
+    // The other warpgroup has issued all MMAs of the previous tile (so every stage before this tile's is filled).
+    if (i > 0) named_bar_sync(my_turn, kConvConsumers);
+    float acc[2][kAcc];
 #pragma unroll
-    for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
-    fence_acc(acc);
+    for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+      for (int k = 0; k < kAcc; ++k) acc[mh][k] = 0.f;
+    fence_acc(acc[0]);
+    fence_acc(acc[1]);
     int prev = -1;
-    const int n_stages = kHalo ? 3 * p.kblocks : k_iters;
     for (int it = 0; it < n_stages; ++it) {
       mbar_wait_u32(full0 + stage * 8, phase);
       wgmma_fence();
@@ -295,93 +350,74 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
         phase ^= 1;
       }
     }
+    // every stage of this tile has been waited for: the other warpgroup may start its tile while these MMAs drain
+    if (tile + static_cast<int>(gridDim.x) < p.num_tiles) named_bar_arrive(their_turn, kConvConsumers);
     wgmma_wait<0>();
-    fence_acc(acc);
+    fence_acc(acc[0]);
+    fence_acc(acc[1]);
     if (prev >= 0) {
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
     }
 
-    // ---------------------------------------------------------------- epilogue
-    // kStats == 3 / kAffine residual: this thread's two rows of the additive tensor (flat mode: tile row == pixel index)
-    const __nv_bfloat16* arow[2] = {nullptr, nullptr};
-    const uint8_t* mrow[2] = {nullptr, nullptr};
-    if ((kStats == 3 || kAffine) && p.mode == 0 && (kStats == 3 || p.add_src != nullptr)) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t grow = static_cast<int64_t>(m_tile) * kBlockM + row0 + 8 * h;
-        if (grow < p.m_rows) {
-          if (kStats == 3) mrow[h] = p.relu_mask + grow * (p.cout >> 3) + ((nb * BLOCK_N) >> 3);
-          if (p.add_mode == 0) {
-            arow[h] = p.add_src + grow * p.cout + nb * BLOCK_N;
-          } else {
-            // compact skip gradient of a stride-2 1x1 projection: only even (h, w) positions carry a value
-            const int wq = static_cast<int>(grow % p.add_w);
-            const int64_t t = grow / p.add_w;
-            const int hq = static_cast<int>(t % p.add_h);
-            const int64_t nq = t / p.add_h;
-            if (((wq | hq) & 1) == 0)
-              arow[h] = p.add_src + ((nq * (p.add_h >> 1) + (hq >> 1)) * (p.add_w >> 1) + (wq >> 1)) * p.cout + nb * BLOCK_N;
-          }
-        }
-      }
-    }
+    // ---------------------------------------------------------------- epilogue (this warpgroup only)
 #pragma unroll
     for (int c = 0; c < kChunks; ++c, ++chunk_ctr) {
-      const int b = chunk_ctr & 1;
-      uint8_t* sbuf = sStage + b * (kBlockM * 128);
-      if (ctid == 0) tma_store_wait_read<1>();  // the store that used this buffer two chunks ago has read it
-      named_bar_sync(1, kConvConsumers);       // ... and every consumer is done with the statistics of that chunk
-      if (kHasY && ctid == 0) {
-        // pre-BN tile of this chunk into Y buffer b (its previous reader, chunk chunk_ctr - 2, is done: barrier above)
-        mbar_arrive_expect_tx(&y_bar[b], static_cast<uint32_t>(p.valid_rows) * 128u);
+      uint8_t* sbuf = sStageW + c * kTileChunkBytes;
+      if (wtid == 0) tma_store_wait_read<kChunks - 1>();  // the store from this buffer one tile ago has read it
+      named_bar_sync(epi_bar, 128);                        // ... and the warpgroup is done with its statistics
+      if (kHasY && wtid == 0) {
+        // pre-BN tile of this chunk (the previous chunk's readers are done: barrier above)
+        mbar_arrive_expect_tx(&y_bar[wg], static_cast<uint32_t>(p.valid_rows) * 128u);
         if (p.mode == 0)
-          tma_load_2d(sY + b * (kBlockM * 128), &tmY, &y_bar[b], nb * BLOCK_N + c * 64, m_tile * kBlockM);
+          tma_load_2d(sYW, &tmY, &y_bar[wg], nb * BLOCK_N + c * 64, m_tile * kBlockM);
         else
-          tma_load_4d(sY + b * (kBlockM * 128), &tmY, &y_bar[b], nb * BLOCK_N + c * 64, w0, h0, n0);
+          tma_load_4d(sYW, &tmY, &y_bar[wg], nb * BLOCK_N + c * 64, w0, h0, n0);
       }
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int i = c * 8 + j;      // 8-column group of the accumulator
-        const int col = i * 8 + cq;   // tile column of v[0] / v[2]
-        float v[4] = {acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3]};
-        if (kAffine) {
-          // out = act(acc * scale[c] + shift[c] [+ residual])
-          const float2 sc = make_float2(__ldg(p.ep_scale + nb * BLOCK_N + col), __ldg(p.ep_scale + nb * BLOCK_N + col + 1));
-          const float2 sh = make_float2(__ldg(p.ep_shift + nb * BLOCK_N + col), __ldg(p.ep_shift + nb * BLOCK_N + col + 1));
+      for (int q = 0; q < 4; ++q) {
+        const int mh = q >> 1, h = q & 1;
+        const int row = 64 * mh + r16 + 8 * h;
+        // This row's residual / skip-gradient words and ReLU-mask bits, all issued before any is used: one memory
+        // latency per row instead of one per 8-column group (the smem stores below would otherwise keep the compiler
+        // from hoisting the loads).  gv[j]: columns 8j + cq, cq + 1; mv: bit k of byte j = column 8j + k.
+        uint32_t gv[8];
+        uint64_t mv = 0ull;
+        if (kStats == 3 || kAffine) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t g = arow[h] != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(arow[h] + col)) : 0u;
-            float f0 = fmaf(v[2 * h], sc.x, sh.x) + __uint_as_float(g << 16);
-            float f1 = fmaf(v[2 * h + 1], sc.y, sh.y) + __uint_as_float(g & 0xFFFF0000u);
-            if (p.ep_act >= 1) f0 = fmaxf(f0, 0.f), f1 = fmaxf(f1, 0.f);
-            if (p.ep_act == 2) f0 = fminf(f0, 6.f), f1 = fminf(f1, 6.f);
-            v[2 * h] = f0;
-            v[2 * h + 1] = f1;
-          }
+          for (int j = 0; j < 8; ++j)
+            gv[j] = arow[q] != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(arow[q] + c * 64 + j * 8 + cq)) : 0u;
+          if (kStats == 3 && mrow[q] != nullptr) mv = __ldg(reinterpret_cast<const unsigned long long*>(mrow[q] + c * 8));
         }
-        if (kStats == 3) {
-          // dz = (main-path gradient + skip gradient) * [block output > 0]
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint32_t g = arow[h] != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(arow[h] + col)) : 0u;
-            const uint32_t m = mrow[h] != nullptr ? static_cast<uint32_t>(__ldg(mrow[h] + (col >> 3))) >> (col & 7) : 0u;
-            v[2 * h] = (m & 1u) ? v[2 * h] + __uint_as_float(g << 16) : 0.f;
-            v[2 * h + 1] = (m & 2u) ? v[2 * h + 1] + __uint_as_float(g & 0xFFFF0000u) : 0.f;
+        for (int j = 0; j < 8; ++j) {
+          const int ig = c * 8 + j;      // 8-column group of the accumulator
+          const int col = ig * 8 + cq;   // tile column of v[0]
+          float v0 = acc[mh][4 * ig + 2 * h], v1 = acc[mh][4 * ig + 2 * h + 1];
+          if (kAffine) {
+            // out = act(acc * scale[c] + shift[c] [+ residual])
+            v0 = fmaf(v0, __ldg(p.ep_scale + nb * BLOCK_N + col), __ldg(p.ep_shift + nb * BLOCK_N + col)) +
+                 __uint_as_float(gv[j] << 16);
+            v1 = fmaf(v1, __ldg(p.ep_scale + nb * BLOCK_N + col + 1), __ldg(p.ep_shift + nb * BLOCK_N + col + 1)) +
+                 __uint_as_float(gv[j] & 0xFFFF0000u);
+            if (p.ep_act >= 1) v0 = fmaxf(v0, 0.f), v1 = fmaxf(v1, 0.f);
+            if (p.ep_act == 2) v0 = fminf(v0, 6.f), v1 = fminf(v1, 6.f);
           }
-        }
-        // bf16 pack + swizzled smem write (16 B chunk j of row r lives at chunk j ^ (r & 7))
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = row0 + 8 * h;
-          uint32_t w = pack_bf16x2(v[2 * h], v[2 * h + 1]);
+          if (kStats == 3) {
+            // dz = (main-path gradient + skip gradient) * [block output > 0]
+            const uint32_t m = static_cast<uint32_t>(mv >> (8 * j + cq));
+            v0 = (m & 1u) ? v0 + __uint_as_float(gv[j] << 16) : 0.f;
+            v1 = (m & 2u) ? v1 + __uint_as_float(gv[j] & 0xFFFF0000u) : 0.f;
+          }
+          // bf16 pack + swizzled smem write (16 B chunk j of row r lives at chunk j ^ (r & 7))
+          uint32_t w = pack_bf16x2(v0, v1);
           if (kStatsOn && row >= p.valid_rows) w = 0u;  // rows past the pixel box: no statistics
           *reinterpret_cast<uint32_t*>(sbuf + row * 128 + ((j ^ (row & 7)) << 4) + (lane & 3) * 4) = w;
         }
       }
       fence_proxy_async_smem();
-      named_bar_sync(1, kConvConsumers);
-      if (ctid == 0) {
+      named_bar_sync(epi_bar, 128);
+      if (wtid == 0) {
         const int ccol = nb * BLOCK_N + c * 64;
         if (p.mode == 0)
           tma_store_2d(&tmD, sbuf, ccol, m_tile * kBlockM);
@@ -391,55 +427,52 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
       }
       if (kStatsOn) {
         // column sums of the bf16 tile just staged (exactly the values BatchNorm will read): one conflict-free LDS.32
-        // per row with precomputed swizzled offsets
-        const uint8_t* srow = sbuf + rg * 16 * 128;
-        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-        if (kStats == 1) {
-#pragma unroll
-          for (int r = 0; r < 16; ++r) {
-            const uint32_t w = *reinterpret_cast<const uint32_t*>(srow + xoff[r & 7] + r * 128);
-            const float lo = __uint_as_float(w << 16);
-            const float hi = __uint_as_float(w & 0xFFFF0000u);
-            s0 += lo;
-            s1 += hi;
-            q0 = fmaf(lo, lo, q0);
-            q1 = fmaf(hi, hi, q1);
-          }
-        } else {
-          const uint8_t* yrow = sY + b * (kBlockM * 128) + rg * 16 * 128;
-          float sc0 = 0.f, sc1 = 0.f, sh0 = 0.f, sh1 = 0.f;
-          if (kStats == 2) {
-            const int gc = nb * BLOCK_N + c * 64 + cp * 2;
-            sc0 = p.bn_scale[gc], sc1 = p.bn_scale[gc + 1];
-            sh0 = p.bn_shift[gc], sh1 = p.bn_shift[gc + 1];
-          }
-          mbar_wait(&y_bar[b], (chunk_ctr >> 1) & 1);
-#pragma unroll
-          for (int r = 0; r < 16; ++r) {
-            const uint32_t w = *reinterpret_cast<const uint32_t*>(srow + xoff[r & 7] + r * 128);
-            const uint32_t u = *reinterpret_cast<const uint32_t*>(yrow + xoff[r & 7] + r * 128);
-            const float y0 = __uint_as_float(u << 16), y1 = __uint_as_float(u & 0xFFFF0000u);
-            float g0 = __uint_as_float(w << 16), g1 = __uint_as_float(w & 0xFFFF0000u);
-            if (kStats == 2) {
-              // dz = g * [y*scale + shift > 0]  (kStats == 3: the staged tile already is dz)
-              g0 = fmaf(y0, sc0, sh0) > 0.f ? g0 : 0.f;
-              g1 = fmaf(y1, sc1, sh1) > 0.f ? g1 : 0.f;
-            }
-            s0 += g0;
-            s1 += g1;
-            q0 = fmaf(g0, y0, q0);
-            q1 = fmaf(g1, y1, q1);
-          }
+        // per row with precomputed swizzled offsets; two 16-row partials per thread, added once
+        float part[2][4];
+        float sc0 = 0.f, sc1 = 0.f, sh0 = 0.f, sh1 = 0.f;
+        if (kStats == 2) {
+          const int gc = nb * BLOCK_N + c * 64 + cp * 2;
+          sc0 = p.bn_scale[gc], sc1 = p.bn_scale[gc + 1];
+          sh0 = p.bn_shift[gc], sh1 = p.bn_shift[gc + 1];
         }
-        sacc[c][0] += s0;
-        sacc[c][1] += s1;
-        sacc[c][2] += q0;
-        sacc[c][3] += q1;
+        if (kHasY) mbar_wait(&y_bar[wg], chunk_ctr & 1);
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+          const uint8_t* srow = sbuf + (rg * 32 + hf * 16) * 128;
+          const uint8_t* yrow = sYW + (rg * 32 + hf * 16) * 128;
+          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+#pragma unroll
+          for (int r = 0; r < 16; ++r) {
+            const uint32_t w = *reinterpret_cast<const uint32_t*>(srow + xoff[r & 7] + r * 128);
+            float g0 = __uint_as_float(w << 16), g1 = __uint_as_float(w & 0xFFFF0000u);
+            if (kStats == 1) {
+              s0 += g0;
+              s1 += g1;
+              q0 = fmaf(g0, g0, q0);
+              q1 = fmaf(g1, g1, q1);
+            } else {
+              const uint32_t u = *reinterpret_cast<const uint32_t*>(yrow + xoff[r & 7] + r * 128);
+              const float y0 = __uint_as_float(u << 16), y1 = __uint_as_float(u & 0xFFFF0000u);
+              if (kStats == 2) {
+                // dz = g * [y*scale + shift > 0]  (kStats == 3: the staged tile already is dz)
+                g0 = fmaf(y0, sc0, sh0) > 0.f ? g0 : 0.f;
+                g1 = fmaf(y1, sc1, sh1) > 0.f ? g1 : 0.f;
+              }
+              s0 += g0;
+              s1 += g1;
+              q0 = fmaf(g0, y0, q0);
+              q1 = fmaf(g1, y1, q1);
+            }
+          }
+          part[hf][0] = s0, part[hf][1] = s1, part[hf][2] = q0, part[hf][3] = q1;
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) sacc[c][k] += part[0][k] + part[1][k];
       }
     }
     if (kStatsOn) {
-      // register accumulators are flushed with global atomics only when the CTA moves to another n-block
-      const int next = tile + gridDim.x;
+      // register accumulators are flushed with global atomics only when this warpgroup moves to another n-block
+      const int next = tile + 2 * gridDim.x;
       if (next >= p.num_tiles || (next % p.n_blocks) != nb) {
 #pragma unroll
         for (int c = 0; c < kChunks; ++c) {
@@ -453,7 +486,7 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
       }
     }
   }
-  if (ctid == 0) tma_store_wait_all<0>();
+  if (wtid == 0) tma_store_wait_all<0>();
 
   if (kStatsOn) {
     // ---- last-CTA tail: every CTA's sums are in L2 once its consumers have fenced and taken a ticket; the CTA
@@ -463,9 +496,9 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
     if (want_tail) {
       unsigned int* counter = (kStats == 1) ? p.fin.counter : p.bfin.counter;
       __threadfence();
-      named_bar_sync(2, kConvConsumers);
+      named_bar_sync(5, kConvConsumers);
       if (ctid == 0) *s_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1 : 0;
-      named_bar_sync(2, kConvConsumers);
+      named_bar_sync(5, kConvConsumers);
       if (*reinterpret_cast<volatile int*>(s_last) != 0) {
         __threadfence();
         for (int c = ctid; c < p.cout; c += kConvConsumers) {
