@@ -85,4 +85,21 @@ void adadelta_step(float* p, const float* g, float* sq, float* acc, void* p16, i
                    cudaStream_t s);
 void cast_f32_to_bf16(const float* x, void* out, int64_t n, cudaStream_t s);
 
+// MobileNetV2 fine-tuning backward with inference-mode BatchNorm (csrc/mobilenet_bwd.cu).
+void relu6_mask_reduce(const void* g1, const void* g2, const void* y, void* dz, float* sum, int64_t M, int C, bool relu6,
+                       cudaStream_t s);
+void dw_dgrad(const void* dz, const float* w, const float* scale, void* dx, int N, int H, int W, int C, int stride,
+              cudaStream_t s);
+void dw_wgrad(const void* dz, const void* x, float* G, int N, int H, int W, int C, int stride, cudaStream_t s);
+void mbv2_stem_wgrad(const uint8_t* x, const void* dz, float* G, int N, int H, int W, int ldc, float mul, float add,
+                     cudaStream_t s);
+// finalize table row (int64): c_real, count, cstride, jstride, w_is_bf16, G off, W off, dgamma off, dbeta off (offsets
+// into the flat buffers), then device pointers scale, invstd, mean, sum_dz
+constexpr int kFtFinalizeFields = 13;
+void mbv2_ft_finalize(const float* params, const void* w16, float* grads, const int64_t* table, int layers, cudaStream_t s);
+// refresh table row (int64): c_real, cp, cin_p (0: no dgrad filter), gamma off, beta off, W off (flat params), then
+// device pointers invstd, mean, scale, shift, wd (bf16 [cin_p, cp] or 0)
+constexpr int kFtRefreshFields = 11;
+void mbv2_ft_refresh(const float* params, const int64_t* table, int layers, cudaStream_t s);
+
 }  // namespace b200

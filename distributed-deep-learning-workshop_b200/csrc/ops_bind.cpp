@@ -452,6 +452,81 @@ void cast_bf16(Tensor x, Tensor out) {
   after();
 }
 
+// ------------------------------------------------------------------------------------------------ MobileNetV2 fine-tuning
+// dz = g1 [+ g2], masked by 0 < y < 6 when relu6; sum[c] += sum_rows dz (sum must be zeroed by the caller).  dz may be g1.
+void relu6_mask_reduce(Tensor g1, OptT g2, Tensor y, Tensor dz, Tensor sum, bool relu6) {
+  const int C = act_channels(y, "y");
+  same_act(g1, y, "g1");
+  same_act(dz, y, "dz");
+  if (g2.has_value()) same_act(*g2, y, "g2");
+  vec(sum, at::kFloat, C, "sum", 1);
+  b200::relu6_mask_reduce(g1.data_ptr(), vp(g2), y.data_ptr(), dz.data_ptr(), sum.data_ptr<float>(), y.numel() / C, C,
+                          relu6, cur());
+  after();
+}
+// NHWC bf16 pair of a depthwise 3x3 (pad 1) layer: input grid x, output grid (H-1)/stride+1; returns C
+static int dw_pair(const Tensor& x, const Tensor& dz, int64_t stride, const char* xname) {
+  TORCH_CHECK(stride == 1 || stride == 2, "stride must be 1 or 2");
+  TORCH_CHECK(x.dim() == 4 && dz.dim() == 4, "depthwise operands are NHWC");
+  const int C = act_channels(x, xname);
+  act_channels(dz, "dz");
+  TORCH_CHECK(dz.size(0) == x.size(0) && dz.size(3) == C && dz.size(1) == (x.size(1) - 1) / stride + 1 &&
+              dz.size(2) == (x.size(2) - 1) / stride + 1, "dz shape does not match the input grid and stride");
+  return C;
+}
+// dx = conv_transpose(dz, scale (.) w) of a depthwise 3x3;  w fp32 [9, C], scale fp32 [C]
+void dw_dgrad(Tensor dz, Tensor w, Tensor scale, Tensor dx, int64_t stride) {
+  const int C = dw_pair(dx, dz, stride, "dx");
+  vec(w, at::kFloat, 9 * (int64_t)C, "w");
+  vec(scale, at::kFloat, C, "scale");
+  b200::dw_dgrad(dz.data_ptr(), w.data_ptr<float>(), scale.data_ptr<float>(), dx.data_ptr(), (int)dx.size(0),
+                 (int)dx.size(1), (int)dx.size(2), C, (int)stride, cur());
+  after();
+}
+// G[9, C] += depthwise 3x3 weight gradient of dz over input x (G zeroed by the caller)
+void dw_wgrad(Tensor dz, Tensor x, Tensor G, int64_t stride) {
+  const int C = dw_pair(x, dz, stride, "x");
+  vec(G, at::kFloat, 9 * (int64_t)C, "G", 4);
+  b200::dw_wgrad(dz.data_ptr(), x.data_ptr(), G.data_ptr<float>(), (int)x.size(0), (int)x.size(1), (int)x.size(2), C,
+                 (int)stride, cur());
+  after();
+}
+// G[27, 32] += weight gradient of the 3x3/2 stem (mbv2_stem) from the uint8 batch and dz bf16 [N, H/2, W/2, ldc]
+void mbv2_stem_wgrad(Tensor x, Tensor dz, Tensor G, double mul, double add) {
+  chk(x, at::kByte, "x");
+  TORCH_CHECK(x.dim() == 4 && x.size(3) == 3 && x.size(1) % 2 == 0 && x.size(2) % 2 == 0,
+              "stem input: uint8 [N, H, W, 3], even H / W");
+  const int ldc = act_channels(dz, "dz");
+  TORCH_CHECK(dz.dim() == 4 && dz.size(0) == x.size(0) && dz.size(1) == x.size(1) / 2 && dz.size(2) == x.size(2) / 2 &&
+              ldc >= 32, "dz: bf16 [N, H/2, W/2, ldc >= 32]");
+  vec(G, at::kFloat, 27 * 32, "G", 4);
+  b200::mbv2_stem_wgrad(x.data_ptr<uint8_t>(), dz.data_ptr(), G.data_ptr<float>(), (int)x.size(0), (int)x.size(1),
+                        (int)x.size(2), ldc, (float)mul, (float)add, cur());
+  after();
+}
+// device table: int64 [layers, fields] on the same device as the flat buffers
+static void ft_table(const Tensor& table, const Tensor& like, int fields) {
+  chk(table, at::kLong, "table");
+  TORCH_CHECK(table.dim() == 2 && table.size(1) == fields && table.size(0) >= 1 && table.size(0) <= 128,
+              "table: int64 [layers (1..128), fields]");
+  TORCH_CHECK(table.device() == like.device(), "table must be on the device of the flat buffers");
+}
+void mbv2_ft_finalize(Tensor params, Tensor w16, Tensor grads, Tensor table) {
+  chk(params, at::kFloat, "params");
+  vec(w16, at::kBFloat16, params.numel(), "w16", 1);
+  vec(grads, at::kFloat, params.numel(), "grads", 1);
+  ft_table(table, params, b200::kFtFinalizeFields);
+  b200::mbv2_ft_finalize(params.data_ptr<float>(), w16.data_ptr(), grads.data_ptr<float>(), table.data_ptr<int64_t>(),
+                         (int)table.size(0), cur());
+  after();
+}
+void mbv2_ft_refresh(Tensor params, Tensor table) {
+  chk(params, at::kFloat, "params");
+  ft_table(table, params, b200::kFtRefreshFields);
+  b200::mbv2_ft_refresh(params.data_ptr<float>(), table.data_ptr<int64_t>(), (int)table.size(0), cur());
+  after();
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -499,4 +574,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cast_bf16", &cast_bf16);
   m.def("launch_count", [] { return g_launches; });
   m.def("reset_launch_count", [] { g_launches = 0; });
+  m.def("relu6_mask_reduce", &relu6_mask_reduce, py::arg("g1"), py::arg("g2"), py::arg("y"), py::arg("dz"), py::arg("sum"),
+        py::arg("relu6") = true);
+  m.def("dw_dgrad", &dw_dgrad);
+  m.def("dw_wgrad", &dw_wgrad);
+  m.def("mbv2_stem_wgrad", &mbv2_stem_wgrad);
+  m.def("mbv2_ft_finalize", &mbv2_ft_finalize);
+  m.def("mbv2_ft_refresh", &mbv2_ft_refresh);
 }

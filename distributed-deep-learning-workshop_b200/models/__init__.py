@@ -23,11 +23,25 @@ CLASSES = ["daisy", "dandelion", "roses", "sunflowers", "tulips"]  # reference P
 
 def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_channels: int = IMG_CHANNELS,
                 num_classes: int = 5, dropout: float = 0.5, arch: Optional[str] = None, batch_size: int = 32,
-                freeze_base: bool = True, device=None, seed: int = 0, **engine_kwargs):
+                freeze_base: bool = True, device=None, seed: int = 0, fine_tune_at: Optional[int] = None,
+                **engine_kwargs):
+    """``fine_tune_at=k`` (MobileNetV2 only, 0..19) fine-tunes ``base.features[k:]`` - conv weights and BatchNorm
+    weight / bias - with every BatchNorm of the base in inference mode (Keras's ``base_model(x, training=False)``).
+    ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only), not
+    Keras's 154 ``base_model.layers``.  ``None`` (default) keeps the base frozen, or fully trainable with
+    training-mode BatchNorm when ``freeze_base=False``; the two options cannot be combined."""
     if isinstance(img_height, float) and img_width == IMG_WIDTH:  # build_model(dropout) positional form
         dropout, img_height = img_height, IMG_HEIGHT
     if img_channels != 3:
         raise ValueError("only 3-channel images are supported")
+    if fine_tune_at is not None:
+        from .mobilenet import check_fine_tune_at
+
+        check_fine_tune_at(fine_tune_at, freeze_base)
+        if arch is None:
+            arch = "mobilenetv2"
+        elif arch not in ("mobilenetv2", "mobilenetv2_head", "mobilenetv2_torch"):
+            raise ValueError("fine_tune_at applies to the MobileNetV2 model only")
     if arch is None:
         arch = "resnet50" if (torch.cuda.is_available() and img_height == img_width and img_height % 32 == 0) else "mobilenetv2"
     if arch == "mobilenetv2_head":   # SURVEY.md 7.1's spelling of the reference's model (frozen MobileNetV2 base + trainable head)
@@ -43,7 +57,7 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
         from .mobilenet_engine import MobileNetV2Engine
 
         return MobileNetV2Engine(batch=batch_size, num_classes=num_classes, device=device, image_size=img_height,
-                                 dropout=dropout, seed=seed)
+                                 dropout=dropout, seed=seed, fine_tune_at=fine_tune_at)
     if arch in ("mobilenetv2", "mobilenetv2_torch"):
         from .mobilenet import FrozenBaseClassifier, MobileNetV2Base
 
@@ -51,7 +65,7 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
         with g:
             torch.manual_seed(seed)
             base = MobileNetV2Base()
-            return FrozenBaseClassifier(base, base.out_channels, num_classes, dropout, freeze_base)
+            return FrozenBaseClassifier(base, base.out_channels, num_classes, dropout, freeze_base, fine_tune_at)
     if arch == "resnet50_torch":
         import torchvision
 

@@ -55,17 +55,41 @@ class MobileNetV2Base(nn.Module):
         return self.features(x)
 
 
+NUM_FEATURE_BLOCKS = 19   # base.features: stem, 17 inverted-residual blocks, last 1x1 conv
+
+
+def check_fine_tune_at(fine_tune_at, freeze_base: bool = True) -> None:
+    if fine_tune_at is None:
+        return
+    if not freeze_base:
+        raise ValueError("fine_tune_at keeps the base's BatchNorm in inference mode; freeze_base=False trains it in "
+                         "training mode - pass one or the other")
+    if isinstance(fine_tune_at, bool) or not isinstance(fine_tune_at, int) or not 0 <= fine_tune_at <= NUM_FEATURE_BLOCKS:
+        raise ValueError(f"fine_tune_at must be an int in 0..{NUM_FEATURE_BLOCKS}, got {fine_tune_at!r}")
+
+
 class FrozenBaseClassifier(nn.Module):
-    """Sequential[base (frozen, inference-mode BN), GlobalAveragePooling2D, Dropout(p), Dense(num_classes)] - logits."""
+    """Sequential[base (frozen, inference-mode BN), GlobalAveragePooling2D, Dropout(p), Dense(num_classes)] - logits.
+
+    ``fine_tune_at=k`` (0..19) is the second phase of Keras's transfer-learning recipe: ``base.features[k:]`` train
+    their conv weights and BatchNorm weight / bias, ``features[:k]`` stay frozen (run under no_grad), and every BatchNorm
+    of the base stays in inference mode (running statistics, never updated), as ``base_model(x, training=False)`` does.
+    ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only), not
+    Keras's 154 ``base_model.layers``."""
 
     def __init__(self, base: nn.Module, feat_channels: int, num_classes: int, dropout: float = 0.5,
-                 freeze_base: bool = True):
+                 freeze_base: bool = True, fine_tune_at=None):
         super().__init__()
+        check_fine_tune_at(fine_tune_at, freeze_base)
         self.base = base
         self.freeze_base = freeze_base
+        self.fine_tune_at = fine_tune_at
         if freeze_base:
             for p in self.base.parameters():
                 p.requires_grad_(False)
+        if fine_tune_at is not None:
+            for p in self.base.features[fine_tune_at:].parameters():
+                p.requires_grad_(True)
         self.dropout = nn.Dropout(dropout)
         self.fc = nn.Linear(feat_channels, num_classes)
 
@@ -76,7 +100,12 @@ class FrozenBaseClassifier(nn.Module):
         return self
 
     def forward(self, x):
-        if self.freeze_base:
+        if self.fine_tune_at is not None:
+            k = self.fine_tune_at
+            with torch.no_grad():
+                f = self.base.features[:k](x)
+            f = self.base.features[k:](f)
+        elif self.freeze_base:
             with torch.no_grad():
                 f = self.base(x)
         else:

@@ -14,6 +14,16 @@ Activations are NHWC bf16 with channel counts padded to multiples of 64 (zero we
 zero).  Only `fc.weight` / `fc.bias` live in the flat fp32 parameter / gradient buffers, so the distributed all-reduce of
 this model is the ~25 KB message the survey describes (SURVEY.md Q11).  Weights use the state-dict names of
 `models.mobilenet.FrozenBaseClassifier`, so checkpoints move freely between the torch module (CPU) and this engine.
+
+`fine_tune_at=k` also trains `base.features[k:]` (conv weights, BatchNorm weight / bias) with every BatchNorm still in
+inference mode, so the forward pass is the one above; only the folded scale / shift of the trainable layers now come
+from the flat parameters (`refresh_derived_weights`, after every optimizer step).  Backward (csrc/mobilenet_bwd.cu)
+runs head -> FC dgrad -> GAP backward -> the trainable layers top-down, per layer: ReLU6 mask / skip add + sum(dz),
+weight gradient G, data gradient with the filter scale (.) W (none for the lowest trainable layer); one finalize launch
+then turns G into dW = scale * G, dgamma = invstd * (<W_c, G_c> - mean * dbeta), dbeta = sum(dz).  Trainable tensors live
+in the flat buffers in backward-completion order (fc, then features.18 down to features.k), each in the layout its
+kernel reads: pointwise [cout_p, cin_p] (zero padding, which gets zero gradient), depthwise [9, Cp], stem [27, 32],
+gamma / beta [c].  The running statistics stay outside the buffers and never change.
 """
 from __future__ import annotations
 
@@ -39,10 +49,18 @@ class MobileNetV2Engine:
     arch = "mobilenetv2"
 
     def __init__(self, batch: int, num_classes: int = 5, device: Optional[torch.device] = None, image_size: int = 224,
-                 dropout: float = 0.5, seed: int = 0, max_ctas: int = 0, bn_eps: float = 1e-5):
+                 dropout: float = 0.5, seed: int = 0, max_ctas: int = 0, bn_eps: float = 1e-5,
+                 fine_tune_at: Optional[int] = None):
+        """``fine_tune_at=k`` (0..19): train ``base.features[k:]`` too, BatchNorm in inference mode (see module doc);
+        ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only)."""
+        from .mobilenet import check_fine_tune_at
+
         ops.require_native()
         if image_size % 32:
             raise ValueError("image_size must be a multiple of 32")
+        check_fine_tune_at(fine_tune_at)
+        self.fine_tune_at = fine_tune_at
+        self._k = 19 if fine_tune_at is None else fine_tune_at
         self.batch, self.num_classes, self.image_size = int(batch), int(num_classes), int(image_size)
         self.dropout, self.seed, self.max_ctas, self.bn_eps = float(dropout), seed, int(max_ctas), bn_eps
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
@@ -51,6 +69,12 @@ class MobileNetV2Engine:
         self.feat_channels = 1280
         specs = [ParamSpec("fc.weight", (self.classes_padded, self.feat_channels), "fc_w"),
                  ParamSpec("fc.bias", (self.num_classes,), "fc_b")]
+        self._layers = self._describe()
+        for kind, conv, bn, cin, cout, _, _, _, feat in reversed(self._layers):
+            if feat >= self._k:
+                wshape = {"stem": (27, 32), "dw": (9, _cp(cin)), "pw": (_cp(cout), _cp(cin))}[kind]
+                specs += [ParamSpec(conv + ".weight", wshape, kind + "_w"), ParamSpec(bn + ".weight", (cout,), "bn_w"),
+                          ParamSpec(bn + ".bias", (cout,), "bn_b")]
         off = 0
         for s in specs:
             s.numel = int(math.prod(s.shape))
@@ -73,13 +97,16 @@ class MobileNetV2Engine:
             torch.manual_seed(seed)
             base = MobileNetV2Base()
             ref = FrozenBaseClassifier(base, base.out_channels, num_classes, dropout, True)
-        self._layers = self._describe()
+        # frozen inference statistics of the trainable layers (fp32 [cp] on the device; set by load_state_dict)
+        self._ft_stats = {bn: (torch.zeros(_cp(cout), device=self.device), torch.zeros(_cp(cout), device=self.device))
+                          for _, _, bn, _, cout, _, _, _, feat in self._layers if feat >= self._k}
         self.load_state_dict(ref.state_dict())
 
     # ------------------------------------------------------------------------------------------------ architecture
     def _describe(self):
-        """[(kind, state-dict prefix of conv, prefix of bn, cin, cout, stride, act, residual?)] in execution order."""
-        L = [("stem", "base.features.0.0", "base.features.0.1", 3, 32, 2, "relu6", False)]
+        """[(kind, state-dict prefix of conv, prefix of bn, cin, cout, stride, act, residual?, index in base.features)]
+        in execution order."""
+        L = [("stem", "base.features.0.0", "base.features.0.1", 3, 32, 2, "relu6", False, 0)]
         cin, idx = 32, 1
         for t, c, n, s in _CFG:
             for i in range(n):
@@ -88,14 +115,14 @@ class MobileNetV2Engine:
                 p = f"base.features.{idx}.conv"
                 k = 0
                 if t != 1:
-                    L.append(("pw", f"{p}.{k}.0", f"{p}.{k}.1", cin, hidden, 1, "relu6", False))
+                    L.append(("pw", f"{p}.{k}.0", f"{p}.{k}.1", cin, hidden, 1, "relu6", False, idx))
                     k += 1
-                L.append(("dw", f"{p}.{k}.0", f"{p}.{k}.1", hidden, hidden, stride, "relu6", False))
+                L.append(("dw", f"{p}.{k}.0", f"{p}.{k}.1", hidden, hidden, stride, "relu6", False, idx))
                 k += 1
-                L.append(("pw", f"{p}.{k}", f"{p}.{k + 1}", hidden, c, 1, "none", stride == 1 and cin == c))
+                L.append(("pw", f"{p}.{k}", f"{p}.{k + 1}", hidden, c, 1, "none", stride == 1 and cin == c, idx))
                 cin = c
                 idx += 1
-        L.append(("pw", f"base.features.{idx}.0", f"base.features.{idx}.1", cin, 1280, 1, "relu6", False))
+        L.append(("pw", f"base.features.{idx}.0", f"base.features.{idx}.1", cin, 1280, 1, "relu6", False, idx))
         return L
 
     # ------------------------------------------------------------------------------------------------ parameters
@@ -123,19 +150,42 @@ class MobileNetV2Engine:
             self.refresh_derived_weights()
 
     def refresh_derived_weights(self) -> None:
-        pass  # the head GEMM reads the flat bf16 copy directly; the base is frozen
+        """Trainable layers: folded scale / shift from gamma / beta and the frozen statistics, bf16 dgrad filters
+        scale (.) W of the pointwise layers, and the FC dgrad filter.  (The head GEMM reads the flat bf16 copy.)"""
+        if self._built and self._ft_stats:
+            self._e.mbv2_ft_refresh(self.params, self._ft_refresh_table)
+        if getattr(self, "_fc_dg", None) is not None:
+            self._e.weight_prep(self.p("fc.weight"), None, self._fc_wd, 1, self.classes_padded, self.feat_channels)
 
     def num_parameters(self) -> int:
         return sum(v.numel() for k, v in self._base_sd.items() if k.endswith(".weight") or k.endswith(".bias")) + \
-            self.trainable_parameters()
+            self.num_classes * self.feat_channels + self.num_classes
 
     def trainable_parameters(self) -> int:
-        return self.num_classes * self.feat_channels + self.num_classes
+        """Unpadded count: the head plus conv weights and BatchNorm weight / bias of base.features[fine_tune_at:]."""
+        n = self.num_classes * self.feat_channels + self.num_classes
+        for kind, _, _, cin, cout, _, _, _, feat in self._layers:
+            if feat >= self._k:
+                n += {"stem": 27 * 32, "dw": 9 * cin, "pw": cout * cin}[kind] + 2 * cout
+        return n
+
+    def _trainable_layers(self):
+        return [lay for lay in self._layers if lay[8] >= self._k]
 
     def state_dict(self) -> Dict[str, torch.Tensor]:
         sd = {k: v.detach().clone().cpu() for k, v in self._base_sd.items()}
         sd["fc.weight"] = self.p("fc.weight")[:self.num_classes].detach().clone().cpu()
         sd["fc.bias"] = self.p("fc.bias").detach().clone().cpu()
+        for kind, conv, bn, cin, cout, *_ in self._trainable_layers():
+            w = self.p(conv + ".weight").detach().cpu()
+            if kind == "stem":   # [27, 32] -> [32, 3, 3, 3]
+                sd[conv + ".weight"] = w.view(3, 3, 3, 32).permute(3, 2, 0, 1).contiguous()
+            elif kind == "dw":   # [9, Cp] -> [C, 1, 3, 3]
+                sd[conv + ".weight"] = w[:, :cin].t().contiguous().view(cin, 1, 3, 3)
+            else:                # [cout_p, cin_p] -> [cout, cin, 1, 1]
+                sd[conv + ".weight"] = w[:cout, :cin].contiguous().view(cout, cin, 1, 1)
+            sd[bn + ".weight"] = self.p(bn + ".weight").detach().clone().cpu()
+            sd[bn + ".bias"] = self.p(bn + ".bias").detach().clone().cpu()
         return sd
 
     def load_state_dict(self, sd: Dict[str, torch.Tensor]) -> None:
@@ -143,9 +193,24 @@ class MobileNetV2Engine:
         self.p("fc.weight").zero_()
         self.p("fc.weight")[:self.num_classes].copy_(sd["fc.weight"].to(self.device, torch.float32))
         self.p("fc.bias").copy_(sd["fc.bias"].to(self.device, torch.float32))
+        for kind, conv, bn, cin, cout, *_ in self._trainable_layers():
+            w, dst = sd[conv + ".weight"].float(), self.p(conv + ".weight")
+            dst.zero_()
+            if kind == "stem":
+                dst.copy_(w.permute(2, 3, 1, 0).reshape(27, 32))
+            elif kind == "dw":
+                dst[:, :cin].copy_(w.view(cin, 9).t())
+            else:
+                dst[:cout, :cin].copy_(w.view(cout, cin))
+            self.p(bn + ".weight").copy_(sd[bn + ".weight"].float())
+            self.p(bn + ".bias").copy_(sd[bn + ".bias"].float())
+            inv, mean = self._ft_stats[bn]
+            inv[:cout].copy_(torch.rsqrt(sd[bn + ".running_var"].float() + self.bn_eps))   # the host fold of _affine
+            mean[:cout].copy_(sd[bn + ".running_mean"].float())
         self._e.cast_bf16(self.params, self.w16)
         if self._built:
             self._load_base_weights()
+            self.refresh_derived_weights()
 
     # ------------------------------------------------------------------------------------------------ build
     def _affine(self, bn: str, c: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -161,6 +226,8 @@ class MobileNetV2Engine:
     def _load_base_weights(self) -> None:
         sd = self._base_sd
         for lay in self._plan:
+            if lay["train"]:
+                continue   # weights live in the flat parameters; scale / shift come from refresh_derived_weights
             kind, conv, bn, cin, cout = lay["kind"], lay["conv"], lay["bn"], lay["cin"], lay["cout"]
             w = sd[conv + ".weight"].float()
             if kind == "stem":   # [32, 3, 3, 3] (co, c, r, s) -> [27, 32] with k = (r*3 + s)*3 + c
@@ -179,6 +246,7 @@ class MobileNetV2Engine:
         if self._built:
             if training and not self._training_built:
                 self._build_head(training=True)
+                self.refresh_derived_weights()
             return self
         if self.grads is None and training:
             self.bind_grad_buffer()
@@ -194,33 +262,106 @@ class MobileNetV2Engine:
         h = S
         x = None
         block_in = None
-        for kind, conv, bn, cin, cout, stride, act, residual in self._layers:
-            lay = dict(kind=kind, conv=conv, bn=bn, cin=cin, cout=cout, stride=stride, act=act)
+        block_src = None   # index in _plan of the layer that wrote block_in
+        for kind, conv, bn, cin, cout, stride, act, residual, feat in self._layers:
+            train = feat >= self._k
+            lay = dict(kind=kind, conv=conv, bn=bn, cin=cin, cout=cout, stride=stride, act=act, train=train)
             ho = h // stride
             out = torch.zeros(N, ho, ho, _cp(cout), **bf)
             lay["scale"], lay["shift"] = torch.ones(_cp(cout), **f32), torch.zeros(_cp(cout), **f32)
             if kind == "stem":
-                lay["w"] = torch.zeros(27, 32, **f32)
+                lay["w"] = self.p(conv + ".weight") if train else torch.zeros(27, 32, **f32)
                 lay["x"], lay["y"] = self.x_u8, out
-                block_in = out
+                block_in, block_src = out, len(self._plan)
             elif kind == "dw":
-                lay["w"] = torch.zeros(9, _cp(cin), **f32)
+                lay["w"] = self.p(conv + ".weight") if train else torch.zeros(9, _cp(cin), **f32)
                 lay["x"], lay["y"] = x, out
             else:
-                lay["w"] = torch.zeros(_cp(cout), _cp(cin), **bf)
+                # a trainable pointwise layer reads the bf16 copy of the flat parameters that the optimizer writes
+                lay["w"] = self.w16v(conv + ".weight") if train else torch.zeros(_cp(cout), _cp(cin), **bf)
+                lay["x"], lay["y"] = x, out
                 res = block_in if residual else None
+                if residual:
+                    lay["res_src"] = block_src
                 lay["op"] = C.ConvForward(x, lay["w"], out, 1, 1, 1, 0, None, None, self.max_ctas,
                                           epilogue=(lay["scale"], lay["shift"], act, res))
                 if act == "none":
-                    block_in = out   # output of an inverted-residual block (linear bottleneck) = the next block's input
+                    # output of an inverted-residual block (linear bottleneck) = the next block's input
+                    block_in, block_src = out, len(self._plan)
             self._plan.append(lay)
             x, h = out, ho
         self.feat = x   # [N, S/32, S/32, 1280]
         self.pooled = torch.zeros(N, self.feat_channels, **bf)
         self._load_base_weights()
-        self._build_head(training)
+        if self._ft_stats:
+            self._ft_refresh_table = self._table([self._refresh_row(lay) for lay in self._plan if lay["train"]])
         self._built = True
+        self._build_head(training)
+        self.refresh_derived_weights()
         return self
+
+    # ------------------------------------------------------------------------------------------------ fine-tuning tables
+    def _table(self, rows: List[List[int]]) -> torch.Tensor:
+        return torch.tensor(rows, dtype=torch.int64).to(self.device)
+
+    def _refresh_row(self, lay: dict) -> List[int]:
+        """mbv2_ft_refresh row: c, cp, cin_p (pointwise dgrad filter) | offsets gamma, beta, W | invstd, mean, scale,
+        shift, dgrad filter pointers."""
+        cout, bn, sp = lay["cout"], lay["bn"], self.spec
+        inv, mean = self._ft_stats[bn]
+        if lay["kind"] == "pw":
+            lay["wd"] = torch.zeros(_cp(lay["cin"]), _cp(cout), device=self.device, dtype=torch.bfloat16)
+        wd = lay.get("wd")
+        return [cout, _cp(cout), _cp(lay["cin"]) if wd is not None else 0, sp[bn + ".weight"].offset,
+                sp[bn + ".bias"].offset, sp[lay["conv"] + ".weight"].offset, inv.data_ptr(), mean.data_ptr(),
+                lay["scale"].data_ptr(), lay["shift"].data_ptr(), wd.data_ptr() if wd is not None else 0]
+
+    def _finalize_row(self, lay: dict) -> List[int]:
+        """mbv2_ft_finalize row: c, elements per channel, channel / element strides of W and G, W is bf16 | offsets G
+        (= W), dgamma, dbeta | scale, invstd, mean, sum(dz) pointers."""
+        kind, cout, bn, sp = lay["kind"], lay["cout"], lay["bn"], self.spec
+        count, cstride, jstride = {"stem": (27, 1, 32), "dw": (9, 1, _cp(cout)),
+                                   "pw": (_cp(lay["cin"]), _cp(lay["cin"]), 1)}[kind]
+        inv, mean = self._ft_stats[bn]
+        off = sp[lay["conv"] + ".weight"].offset
+        return [cout, count, cstride, jstride, int(kind == "pw"), off, off, sp[bn + ".weight"].offset,
+                sp[bn + ".bias"].offset, lay["scale"].data_ptr(), inv.data_ptr(), mean.data_ptr(),
+                lay["sum"].data_ptr()]
+
+    def _build_backward(self) -> None:
+        """Gradient buffers and plans of the trainable base layers (training build with fine_tune_at <= 18)."""
+        N, ncp, mc, F = self.batch, self.classes_padded, self.max_ctas, self.feat_channels
+        bf = dict(device=self.device, dtype=torch.bfloat16)
+        self.dpooled = torch.zeros(N, F, **bf)
+        self._fc_wd = torch.zeros(F, ncp, **bf)
+        self._fc_dg = C.ConvDgrad(self.dlogits16.view(N, 1, 1, ncp), self.p("fc.weight").view(1, ncp, F),
+                                  self.dpooled.view(N, 1, 1, F), 1, 1, 1, 0, mc, wbuf=self._fc_wd)
+        train = [i for i, lay in enumerate(self._plan) if lay["train"]]
+        self._ft_lowest = train[0]
+        self._ft_sums = torch.zeros(sum(_cp(self._plan[i]["cout"]) for i in train), device=self.device)
+        off = 0
+        for i in train:
+            lay = self._plan[i]
+            cp = _cp(lay["cout"])
+            lay["sum"] = self._ft_sums[off:off + cp]
+            off += cp
+            lay["g"] = torch.zeros_like(lay["y"])   # gradient at the output; turned into dz in place
+            lay["g2"] = None
+        for i in train:
+            lay = self._plan[i]
+            if "res_src" in lay and self._plan[lay["res_src"]]["train"]:
+                self._plan[lay["res_src"]]["g2"] = lay["g"]   # skip gradient = dz of the block's linear output
+            if lay["kind"] == "pw":
+                w = self.p(lay["conv"] + ".weight")
+                # the wgrad GEMM takes Cout == 64 or a multiple of 128: 128*a + 64 output channels run as two GEMMs
+                G, cp = self.g(lay["conv"] + ".weight"), _cp(lay["cout"])
+                cuts = [0, cp] if cp == 64 or cp % 128 == 0 else [0, cp - 64, cp]
+                lay["wg"] = [C.ConvWgrad(lay["g"][..., a:b], lay["x"], G[a:b], 1, 1, 1, 0, 0, mc, 0)
+                             for a, b in zip(cuts, cuts[1:])]
+                if i > self._ft_lowest:
+                    lay["dg"] = C.ConvDgrad(lay["g"], w.view(1, *w.shape), self._plan[i - 1]["g"], 1, 1, 1, 0, mc,
+                                            wbuf=lay["wd"])
+        self._ft_finalize_table = self._table([self._finalize_row(self._plan[i]) for i in train])
 
     def _build_head(self, training: bool) -> None:
         N, ncp, mc = self.batch, self.classes_padded, self.max_ctas
@@ -235,6 +376,8 @@ class MobileNetV2Engine:
             self.dlogits16 = torch.zeros(N, ncp, **bf)
             self._fc_wg = C.ConvWgrad(self.dlogits16.view(N, 1, 1, ncp), self.pooled.view(N, 1, 1, self.feat_channels),
                                       self.g("fc.weight"), 1, 1, 1, 0, 0, mc, 0)
+            if self._ft_stats:
+                self._build_backward()
             self._training_built = True
 
     # ------------------------------------------------------------------------------------------------ forward / backward
@@ -256,13 +399,39 @@ class MobileNetV2Engine:
                           self.dlogits16 if (training and self._training_built) else None, self.loss_rows, self.stats, 1.0 / N)
 
     def backward(self) -> None:
-        """Only the Dense head is trainable: its weight / bias gradients (the base receives no gradient)."""
+        """Dense head weight / bias gradients; with fine_tune_at <= 18 also those of base.features[fine_tune_at:]."""
         e = self._e
         e.zero_(self.grads)
         self._fc_wg.run()
         e.fc_bias_grad(self.dlogits16, self.g("fc.bias"))
+        if self._ft_stats:
+            self._backward_base()
         if self.grad_hook is not None:
             self.grad_hook(0, self.flat_numel)
+
+    def _backward_base(self) -> None:
+        e = self._e
+        e.zero_(self._ft_sums)
+        self._fc_dg.run()
+        e.gap_bwd(self.dpooled, self._plan[-1]["g"], self.dropout, self._drop_seed)
+        for i in range(len(self._plan) - 1, self._ft_lowest - 1, -1):
+            lay = self._plan[i]
+            g, kind = lay["g"], lay["kind"]
+            e.relu6_mask_reduce(g, lay["g2"], lay["y"], g, lay["sum"], lay["act"] == "relu6")
+            G = self.g(lay["conv"] + ".weight")
+            if kind == "pw":
+                for op in lay["wg"]:
+                    op.run()
+            elif kind == "dw":
+                e.dw_wgrad(g, lay["x"], G, lay["stride"])
+            else:
+                e.mbv2_stem_wgrad(lay["x"], g, G, 1.0 / 127.5, -1.0)
+            if i > self._ft_lowest:
+                if kind == "pw":
+                    lay["dg"].run()
+                else:
+                    e.dw_dgrad(g, lay["w"], lay["scale"], self._plan[i - 1]["g"], lay["stride"])
+        e.mbv2_ft_finalize(self.params, self.w16, self.grads, self._ft_finalize_table)
 
     # ------------------------------------------------------------------------------------------------ utilities
     def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None) -> None:

@@ -34,7 +34,7 @@ CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC"]
 EXTENSIONS: Dict[str, List[str]] = {
     "_b200_conv": ["conv_igemm.cu", "conv_wgrad.cu", "stem.cu", "tmap.cpp", "conv_bind.cpp"],
     "_b200_probe": ["tma_probe.cu", "tmap.cpp", "probe_bind.cpp"],   # hardware probe, not on any hot path
-    "_b200_ops": ["elementwise.cu", "head_stem.cu", "mobilenet.cu", "optim.cu", "ops_bind.cpp"],
+    "_b200_ops": ["elementwise.cu", "head_stem.cu", "mobilenet.cu", "optim.cu", "mobilenet_bwd.cu", "ops_bind.cpp"],
     "_b200_comm": ["allreduce.cu", "comm_bind.cpp"],
     "_b200_loader": ["ring_loader.cpp"],
     "_b200_jpeg": ["jpeg_decode.cpp", "jpeg_resize.cu"],   # nvJPEG (library) decode + our batched resize kernel

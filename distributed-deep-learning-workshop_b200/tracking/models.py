@@ -11,13 +11,16 @@ import torch
 
 def _describe(model) -> dict:
     if hasattr(model, "param_specs"):  # native engines (ResNet50Engine, MobileNetV2Engine)
-        return {"arch": getattr(model, "arch", "resnet50"), "num_classes": model.num_classes, "image_size": model.image_size,
+        desc = {"arch": getattr(model, "arch", "resnet50"), "num_classes": model.num_classes, "image_size": model.image_size,
                 "dropout": model.dropout, "batch": model.batch, "engine": True}
+        if desc["arch"] == "mobilenetv2":
+            desc["fine_tune_at"] = model.fine_tune_at
+        return desc
     from ..models.mobilenet import FrozenBaseClassifier
 
     if isinstance(model, FrozenBaseClassifier):
         return {"arch": "mobilenetv2", "num_classes": model.fc.out_features, "dropout": model.dropout.p,
-                "freeze_base": model.freeze_base}
+                "freeze_base": model.freeze_base, "fine_tune_at": model.fine_tune_at}
     return {"arch": "pickle"}
 
 
@@ -71,10 +74,11 @@ def load_model(model_uri: str, batch_size: Optional[int] = None, device=None):
             model.load_state_dict(sd, strict=False)
     elif desc.get("engine") and torch.cuda.is_available():  # saved from the native MobileNetV2 engine
         model = build_model(desc["image_size"], desc["image_size"], 3, desc["num_classes"], desc["dropout"],
-                            arch="mobilenetv2", batch_size=batch_size or desc["batch"], device=device)
+                            arch="mobilenetv2", batch_size=batch_size or desc["batch"], device=device,
+                            fine_tune_at=desc.get("fine_tune_at"))
         model.load_state_dict(sd)
     else:
         model = build_model(num_classes=desc["num_classes"], dropout=desc["dropout"], arch="mobilenetv2_torch",
-                            freeze_base=desc.get("freeze_base", True))
+                            freeze_base=desc.get("freeze_base", True), fine_tune_at=desc.get("fine_tune_at"))
         model.load_state_dict(sd)
     return Trainer(model, device=device)
