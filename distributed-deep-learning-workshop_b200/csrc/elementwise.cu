@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "hash.cuh"
 #include "ops_api.h"
 
 namespace b200 {
@@ -699,12 +700,7 @@ void maxpool_bwd(const void* idx, const void* g1, const void* g2, void* dx, int 
 }
 
 // ------------------------------------------------------------------------------------------------ global avg pool
-// x [N, HW, C] -> out [N, C]  (optionally with inverted-dropout mask from a counter-based hash RNG)
-__device__ __forceinline__ uint32_t hash_u32(uint32_t a, uint32_t b, uint32_t c) {
-  uint32_t h = a * 0x9E3779B1u ^ (b + 0x7F4A7C15u) * 0x85EBCA77u ^ (c + 0x165667B1u) * 0xC2B2AE3Du;
-  h ^= h >> 15; h *= 0x2C1B3C6Du; h ^= h >> 12; h *= 0x297A2D39u; h ^= h >> 15;
-  return h;
-}
+// x [N, HW, C] -> out [N, C]  (optionally with inverted-dropout mask from a counter-based hash RNG, csrc/hash.cuh)
 __global__ void gap_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out, int N, int HW,
                                int C, float keep_scale, uint32_t keep_thresh, uint32_t seed_lo, uint32_t seed_hi) {
   const int cvec = C / 8;

@@ -102,4 +102,17 @@ void mbv2_ft_finalize(const float* params, const void* w16, float* grads, const 
 constexpr int kFtRefreshFields = 11;
 void mbv2_ft_refresh(const float* params, const int64_t* table, int layers, cudaStream_t s);
 
+// Random augmentation of the uint8 NHWC training batch (csrc/augment.cu).  params: int32 [N, 8] per image =
+// Q16.16 a00 a01 b0 a10 a11 b1, flip bits, 0;  rot_table: int32 [2^kAugRotBits][2] Q16.16 (cos, sin);  step: one int32 in
+// device memory;  zq / txq / tyq: Q16.16 zoom half-range and translation half-ranges in pixels.  H, W <= kAugMaxSide keeps
+// every source coordinate inside int32.
+constexpr int kAugParamFields = 8;
+constexpr int kAugRotBits = 12;
+constexpr int kAugMaxSide = 2048;
+constexpr int kAugWarpMaxBlocks = 132 * 8;   // upper bound of the warp's grid (it launches one wave of resident blocks)
+void augment_params(int32_t* params, const int32_t* step, const int32_t* rot_table, int N, int H, int W, uint32_t key,
+                    int flip_mode, int32_t zq, int32_t txq, int32_t tyq, cudaStream_t s);
+void augment_warp(const uint8_t* x, uint8_t* out, const int32_t* params, int N, int H, int W, bool reflect, int fill,
+                  cudaStream_t s);
+
 }  // namespace b200

@@ -527,6 +527,56 @@ void mbv2_ft_refresh(Tensor params, Tensor table) {
   after();
 }
 
+// ------------------------------------------------------------------------------------------------ augmentation
+// params int32 [N, 8] (16-byte aligned rows) of a batch of N images of H x W
+static void aug_params_table(const Tensor& params, int64_t N, const char* name) {
+  chk(params, at::kInt, name);
+  TORCH_CHECK(params.dim() == 2 && params.size(1) == b200::kAugParamFields && params.size(0) == N,
+              name, " must be int32 [N, 8] for the batch's N images");
+  aligned(params, 16, name);
+}
+static void aug_side(int64_t H, int64_t W) {
+  TORCH_CHECK(H >= 1 && W >= 1 && H <= b200::kAugMaxSide && W <= b200::kAugMaxSide,
+              "augmentation: image sides must be in 1..2048");
+}
+// params[n] = transform of image n for the step held in `step` (int32 [1] on the device); see csrc/augment.cu
+void augment_params(Tensor params, Tensor step, Tensor rot_table, int64_t H, int64_t W, int64_t key, int64_t flip_mode,
+                    int64_t zq, int64_t txq, int64_t tyq) {
+  TORCH_CHECK(params.dim() == 2 && params.size(0) >= 1, "params must be int32 [N, 8] with N >= 1");
+  aug_params_table(params, params.size(0), "params");
+  vec(step, at::kInt, 1, "step", 4);
+  vec(rot_table, at::kInt, 2 << b200::kAugRotBits, "rot_table", 8);
+  TORCH_CHECK(step.device() == params.device() && rot_table.device() == params.device(),
+              "step and rot_table must be on the device of params");
+  aug_side(H, W);
+  TORCH_CHECK(key >= 0 && key <= 0xFFFFFFFFLL, "key must be a uint32");
+  TORCH_CHECK(flip_mode >= 0 && flip_mode <= 3, "flip_mode: bit 0 horizontal, bit 1 vertical");
+  TORCH_CHECK(zq >= 0 && zq < 65536, "zq: Q16.16 zoom factor in [0, 1)");
+  TORCH_CHECK(txq >= 0 && txq <= W * 65536 && tyq >= 0 && tyq <= H * 65536,
+              "txq / tyq: Q16.16 translation in [0, W] / [0, H] pixels");
+  b200::augment_params(params.data_ptr<int32_t>(), step.data_ptr<int32_t>(), rot_table.data_ptr<int32_t>(),
+                       (int)params.size(0), (int)H, (int)W, (uint32_t)key, (int)flip_mode, (int32_t)zq, (int32_t)txq,
+                       (int32_t)tyq, cur());
+  after();
+}
+// out = bilinear warp of x (uint8 [N, H, W, 3]) by the per-image maps in params; fill_mode "reflect" or "constant"
+void augment_warp(Tensor x, Tensor out, Tensor params, std::string fill_mode, int64_t fill_value) {
+  chk(x, at::kByte, "x");
+  chk(out, at::kByte, "out");
+  TORCH_CHECK(x.dim() == 4 && x.size(3) == 3 && x.size(0) >= 1, "x must be uint8 [N, H, W, 3]");
+  TORCH_CHECK(out.sizes() == x.sizes(), "out must have the shape of x");
+  TORCH_CHECK(out.device() == x.device() && params.device() == x.device(), "x, out and params must share a device");
+  TORCH_CHECK(out.data_ptr() != x.data_ptr(), "augment_warp cannot run in place");
+  aligned(out, 16, "out");
+  aug_side(x.size(1), x.size(2));
+  aug_params_table(params, x.size(0), "params");
+  TORCH_CHECK(fill_mode == "reflect" || fill_mode == "constant", "fill_mode must be 'reflect' or 'constant'");
+  TORCH_CHECK(fill_value >= 0 && fill_value <= 255, "fill_value must be a uint8");
+  b200::augment_warp(x.data_ptr<uint8_t>(), out.data_ptr<uint8_t>(), params.data_ptr<int32_t>(), (int)x.size(0),
+                     (int)x.size(1), (int)x.size(2), fill_mode == "reflect", (int)fill_value, cur());
+  after();
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -581,4 +631,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mbv2_stem_wgrad", &mbv2_stem_wgrad);
   m.def("mbv2_ft_finalize", &mbv2_ft_finalize);
   m.def("mbv2_ft_refresh", &mbv2_ft_refresh);
+  m.def("augment_params", &augment_params, py::arg("params"), py::arg("step"), py::arg("rot_table"), py::arg("H"),
+        py::arg("W"), py::arg("key"), py::arg("flip_mode"), py::arg("zq"), py::arg("txq"), py::arg("tyq"));
+  m.def("augment_warp", &augment_warp, py::arg("x"), py::arg("out"), py::arg("params"), py::arg("fill_mode"),
+        py::arg("fill_value"));
 }

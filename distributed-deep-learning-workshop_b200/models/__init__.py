@@ -16,6 +16,7 @@ from typing import Optional
 
 import torch
 
+from .augment import Augmentation, check_augmentation
 from .preprocess import (IMG_CHANNELS, IMG_HEIGHT, IMG_WIDTH, decode_batch, decode_image, preprocess, preprocess_tensor)
 
 CLASSES = ["daisy", "dandelion", "roses", "sunflowers", "tulips"]  # reference P2/03:62
@@ -24,16 +25,21 @@ CLASSES = ["daisy", "dandelion", "roses", "sunflowers", "tulips"]  # reference P
 def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_channels: int = IMG_CHANNELS,
                 num_classes: int = 5, dropout: float = 0.5, arch: Optional[str] = None, batch_size: int = 32,
                 freeze_base: bool = True, device=None, seed: int = 0, fine_tune_at: Optional[int] = None,
-                **engine_kwargs):
+                augmentation: Optional[Augmentation] = None, **engine_kwargs):
     """``fine_tune_at=k`` (MobileNetV2 only, 0..19) fine-tunes ``base.features[k:]`` - conv weights and BatchNorm
     weight / bias - with every BatchNorm of the base in inference mode (Keras's ``base_model(x, training=False)``).
     ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only), not
     Keras's 154 ``base_model.layers``.  ``None`` (default) keeps the base frozen, or fully trainable with
-    training-mode BatchNorm when ``freeze_base=False``; the two options cannot be combined."""
+    training-mode BatchNorm when ``freeze_base=False``; the two options cannot be combined.
+
+    ``augmentation`` (`Augmentation`): random flip / rotation / zoom / translation of every training batch (Keras's
+    augmentation layers in front of the model), on the device for the native engines; ``evaluate`` / ``predict`` never
+    augment.  ``None`` (default) leaves every path unchanged.  Not available for ``arch='resnet50_torch'``."""
     if isinstance(img_height, float) and img_width == IMG_WIDTH:  # build_model(dropout) positional form
         dropout, img_height = img_height, IMG_HEIGHT
     if img_channels != 3:
         raise ValueError("only 3-channel images are supported")
+    augmentation = check_augmentation(augmentation)
     if fine_tune_at is not None:
         from .mobilenet import check_fine_tune_at
 
@@ -50,14 +56,14 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
         from .resnet_engine import ResNet50Engine
 
         return ResNet50Engine(batch=batch_size, num_classes=num_classes, device=device, image_size=img_height,
-                              dropout=dropout, seed=seed, **engine_kwargs)
+                              dropout=dropout, seed=seed, augmentation=augmentation, **engine_kwargs)
     if arch == "mobilenetv2" and freeze_base and torch.cuda.is_available() and img_height == img_width and img_height % 32 == 0 \
             and (device is None or torch.device(device).type == "cuda"):
         # the reference's own model on native kernels (frozen base = inference-mode layers; trainable Dense head)
         from .mobilenet_engine import MobileNetV2Engine
 
         return MobileNetV2Engine(batch=batch_size, num_classes=num_classes, device=device, image_size=img_height,
-                                 dropout=dropout, seed=seed, fine_tune_at=fine_tune_at)
+                                 dropout=dropout, seed=seed, fine_tune_at=fine_tune_at, augmentation=augmentation)
     if arch in ("mobilenetv2", "mobilenetv2_torch"):
         from .mobilenet import FrozenBaseClassifier, MobileNetV2Base
 
@@ -65,8 +71,11 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
         with g:
             torch.manual_seed(seed)
             base = MobileNetV2Base()
-            return FrozenBaseClassifier(base, base.out_channels, num_classes, dropout, freeze_base, fine_tune_at)
+            return FrozenBaseClassifier(base, base.out_channels, num_classes, dropout, freeze_base, fine_tune_at,
+                                        augmentation=augmentation, augmentation_seed=seed)
     if arch == "resnet50_torch":
+        if augmentation is not None:
+            raise ValueError("arch='resnet50_torch' is the plain torchvision module and takes no augmentation")
         import torchvision
 
         with torch.random.fork_rng(devices=[]):
@@ -75,5 +84,5 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
     raise ValueError(f"unknown arch {arch!r}")
 
 
-__all__ = ["build_model", "preprocess", "preprocess_tensor", "decode_image", "decode_batch", "CLASSES", "IMG_HEIGHT", "IMG_WIDTH",
+__all__ = ["build_model", "Augmentation", "preprocess", "preprocess_tensor", "decode_image", "decode_batch", "CLASSES", "IMG_HEIGHT", "IMG_WIDTH",
            "IMG_CHANNELS"]

@@ -75,12 +75,20 @@ class FrozenBaseClassifier(nn.Module):
     their conv weights and BatchNorm weight / bias, ``features[:k]`` stay frozen (run under no_grad), and every BatchNorm
     of the base stays in inference mode (running statistics, never updated), as ``base_model(x, training=False)`` does.
     ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only), not
-    Keras's 154 ``base_model.layers``."""
+    Keras's 154 ``base_model.layers``.
+
+    ``augmentation`` (`models.augment.Augmentation`) is applied by the trainer's module backend to the uint8 batch of
+    every training step (the reference implementation of the engines' kernels, keyed by ``augmentation_seed`` and the
+    rank); the module's own forward never augments."""
 
     def __init__(self, base: nn.Module, feat_channels: int, num_classes: int, dropout: float = 0.5,
-                 freeze_base: bool = True, fine_tune_at=None):
+                 freeze_base: bool = True, fine_tune_at=None, augmentation=None, augmentation_seed: int = 0):
+        from .augment import check_augmentation
+
         super().__init__()
         check_fine_tune_at(fine_tune_at, freeze_base)
+        self.augmentation = check_augmentation(augmentation)
+        self.augmentation_seed = int(augmentation_seed)
         self.base = base
         self.freeze_base = freeze_base
         self.fine_tune_at = fine_tune_at

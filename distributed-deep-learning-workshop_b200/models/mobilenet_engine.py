@@ -34,7 +34,7 @@ import torch
 
 from .. import ops
 from ..ops import conv as C
-from .resnet_engine import ParamSpec, _align
+from .resnet_engine import ParamSpec, _align, _augmenter
 
 _CFG = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2), (6, 320, 1, 1)]
 
@@ -50,12 +50,17 @@ class MobileNetV2Engine:
 
     def __init__(self, batch: int, num_classes: int = 5, device: Optional[torch.device] = None, image_size: int = 224,
                  dropout: float = 0.5, seed: int = 0, max_ctas: int = 0, bn_eps: float = 1e-5,
-                 fine_tune_at: Optional[int] = None):
+                 fine_tune_at: Optional[int] = None, augmentation=None):
         """``fine_tune_at=k`` (0..19): train ``base.features[k:]`` too, BatchNorm in inference mode (see module doc);
-        ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only)."""
+        ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only).
+        ``augmentation`` (`models.augment.Augmentation`): random flip / rotation / zoom / translation of the input batch
+        in every training step, on the device; evaluation and inference never apply it."""
+        from .augment import check_augmentation
         from .mobilenet import check_fine_tune_at
 
         ops.require_native()
+        self.augmentation = check_augmentation(augmentation)
+        self._augmenter = None
         if image_size % 32:
             raise ValueError("image_size must be a multiple of 32")
         check_fine_tune_at(fine_tune_at)
@@ -378,14 +383,17 @@ class MobileNetV2Engine:
                                       self.g("fc.weight"), 1, 1, 1, 0, 0, mc, 0)
             if self._ft_stats:
                 self._build_backward()
+            self._augmenter = _augmenter(self, self.x_u8)
             self._training_built = True
 
     # ------------------------------------------------------------------------------------------------ forward / backward
     def forward(self, training: bool = True) -> None:
         e, N = self._e, self.batch
+        if training and self._augmenter is not None:
+            self._augmenter.run()
         for lay in self._plan:
             if lay["kind"] == "stem":
-                e.mbv2_stem(lay["x"], lay["w"], lay["scale"], lay["shift"], lay["y"], 1.0 / 127.5, -1.0)
+                e.mbv2_stem(self._stem_input(training), lay["w"], lay["scale"], lay["shift"], lay["y"], 1.0 / 127.5, -1.0)
             elif lay["kind"] == "dw":
                 e.dwconv3x3(lay["x"], lay["w"], lay["scale"], lay["shift"], lay["y"], lay["stride"])
             else:
@@ -425,7 +433,7 @@ class MobileNetV2Engine:
             elif kind == "dw":
                 e.dw_wgrad(g, lay["x"], G, lay["stride"])
             else:
-                e.mbv2_stem_wgrad(lay["x"], g, G, 1.0 / 127.5, -1.0)
+                e.mbv2_stem_wgrad(self._stem_input(True), g, G, 1.0 / 127.5, -1.0)
             if i > self._ft_lowest:
                 if kind == "pw":
                     lay["dg"].run()
@@ -433,7 +441,16 @@ class MobileNetV2Engine:
                     e.dw_dgrad(g, lay["w"], lay["scale"], self._plan[i - 1]["g"], lay["stride"])
         e.mbv2_ft_finalize(self.params, self.w16, self.grads, self._ft_finalize_table)
 
+    def _stem_input(self, training: bool) -> torch.Tensor:
+        """uint8 batch the stem reads: the augmented copy in training steps, x_u8 otherwise."""
+        return self._augmenter.out if (training and self._augmenter is not None) else self.x_u8
+
     # ------------------------------------------------------------------------------------------------ utilities
+    def set_augment_step(self, t: int) -> None:
+        """Step word the next training forward's augmentation reads (the optimizer's step counter)."""
+        if self._augmenter is not None:
+            self._augmenter.set_step(t)
+
     def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None) -> None:
         self.x_u8.copy_(x_u8.view(self.x_u8.shape), non_blocking=True)
         if labels is not None:

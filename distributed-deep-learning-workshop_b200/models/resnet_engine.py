@@ -64,6 +64,17 @@ def _align(n: int, a: int = 64) -> int:
     return (n + a - 1) // a * a
 
 
+def _augmenter(engine, x_u8: torch.Tensor):
+    """The engine's device augmenter over its input buffer (None without an augmentation): it owns the augmented-input
+    buffer and the device step word, keyed by the engine's seed and this process's data-parallel rank."""
+    if engine.augmentation is None:
+        return None
+    from ..parallel import core as _core
+    from .augment import DeviceAugmenter
+
+    return DeviceAugmenter(engine.augmentation, x_u8, engine.seed, _core.rank())
+
+
 def resnet50_blocks(image_size: int = 224) -> List[BlockSpec]:
     cfg = [(64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)]
     blocks = []
@@ -88,8 +99,14 @@ class ResNet50Engine:
                  seed: int = 0, max_ctas: int = 0, zero_init_residual: bool = True, native_stem: bool = True,
                  overlap_wgrad: bool = True, wgrad_smem_budget: int = 0, fuse_bwd_reduce: bool = True,
                  fuse_bn_coeffs: bool = False, fuse_block_grad: Optional[bool] = None,
-                 fuse_stem_bwd: Optional[bool] = None):
+                 fuse_stem_bwd: Optional[bool] = None, augmentation=None):
+        """``augmentation`` (`models.augment.Augmentation`): random flip / rotation / zoom / translation of the input
+        batch in every training step, on the device (see `models.augment`); evaluation and inference never apply it."""
+        from .augment import check_augmentation
+
         ops.require_native()
+        self.augmentation = check_augmentation(augmentation)
+        self._augmenter = None
         self.zero_init_residual = zero_init_residual
         self.native_stem = native_stem
         # experimental: run every weight-gradient GEMM on a side stream so it overlaps the (DRAM-bound) BatchNorm
@@ -284,6 +301,9 @@ class ResNet50Engine:
         self.x_u8 = torch.zeros(N, S, S, 3, device=dev, dtype=torch.uint8)
         self.labels = torch.zeros(N, device=dev, dtype=torch.int64)
         self.x16 = torch.zeros(N, S, S, 3, **bf)
+        # training steps read the augmented copy of x_u8 (every stem reader below); eval reads x_u8 itself
+        self._augmenter = _augmenter(self, self.x_u8) if training else None
+        x_train = self._augmenter.out if self._augmenter is not None else self.x_u8
         self.stats = torch.zeros(2, **f32)          # [sum loss, correct]
         self.logits = torch.zeros(N, self.num_classes, **f32)  # fp32 logits (+bias) for predict(); written by the CE kernel
         self.loss_rows = torch.zeros(N, **f32)
@@ -314,6 +334,8 @@ class ResNet50Engine:
         if self.native_stem:
             self._stem_w16 = torch.zeros(64, 192, **bf)
             self._stem_fwd = C.StemForward(self.x_u8, self._stem_w16, self.y0, w0["sum"], w0["sqsum"], max_ctas=self.max_ctas)
+            self._stem_fwd_train = self._stem_fwd if x_train is self.x_u8 else \
+                C.StemForward(x_train, self._stem_w16, self.y0, w0["sum"], w0["sqsum"], max_ctas=self.max_ctas)
         else:
             self._stem_w = torch.zeros(64, 3, 7, 7, **bf).contiguous(memory_format=torch.channels_last)
         self._refresh_stem_weight()
@@ -534,7 +556,7 @@ class ResNet50Engine:
                                       self.dpooled.view(N, 1, 1, 2048), 1, 1, 1, 0, mc, wbufs=wd_views("fc"))
             if self.native_stem:
                 dy0 = self._scr["dzA"][:self.y0.numel()].view(self.y0.shape)
-                self._stem_wg = C.StemWgrad(self.x_u8, dy0, self.g("conv1.weight").view(-1), max_ctas=self.max_ctas)
+                self._stem_wg = C.StemWgrad(x_train, dy0, self.g("conv1.weight").view(-1), max_ctas=self.max_ctas)
         self._training_built = training
         self._built = True
         self.sync_weights()
@@ -584,11 +606,14 @@ class ResNet50Engine:
             self._tail_state = training
         if training and self.fuse_bn_coeffs:
             e.zero_(self._bn_fwd_sums)  # nobody zeroes them after use on the fused path
+        augment = training and self._augmenter is not None
+        if augment:
+            self._augmenter.run()
         if self.native_stem:
             # 7x7/2 stem on the tensor cores straight from the uint8 batch (normalisation + BN statistics fused)
-            self._stem_fwd.run()
+            (self._stem_fwd_train if training else self._stem_fwd).run()
         else:
-            e.preprocess_u8(self.x_u8, self.x16, 1.0 / 127.5, -1.0)
+            e.preprocess_u8(self._augmenter.out if augment else self.x_u8, self.x16, 1.0 / 127.5, -1.0)
             y0 = torch.nn.functional.conv2d(self.x16.permute(0, 3, 1, 2), self._stem_w, stride=2, padding=3)
             self.y0.copy_(y0.permute(0, 2, 3, 1))
             e.channel_stats(self.y0, w0["sum"], w0["sqsum"])
@@ -799,6 +824,11 @@ class ResNet50Engine:
         if labels is not None:
             self.labels.copy_(labels, non_blocking=True)
 
+    def set_augment_step(self, t: int) -> None:
+        """Step word the next training forward's augmentation reads (the optimizer's step counter)."""
+        if self._augmenter is not None:
+            self._augmenter.set_step(t)
+
     def loss_and_acc(self) -> Tuple[float, float]:
         s = self.stats.tolist()
         return s[0] / self.batch, s[1] / self.batch
@@ -947,6 +977,10 @@ class EngineTrainStep:
             self.capture()
         self.optimizer.begin_step()
         self.engine._step_count += 1
+        if getattr(self.engine, "augmentation", None) is not None:
+            # written to device memory before every replay: the augmentation draws depend on the step, and a graph
+            # captures kernel arguments by value (warm-up in capture() never writes the word, so step 1 sees t = 1)
+            self.engine.set_augment_step((self.optimizer.opt if self._dist else self.optimizer).t)
         if self.graph is not None:
             self.graph.replay()
         else:

@@ -34,7 +34,8 @@ CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC"]
 EXTENSIONS: Dict[str, List[str]] = {
     "_b200_conv": ["conv_igemm.cu", "conv_wgrad.cu", "stem.cu", "tmap.cpp", "conv_bind.cpp"],
     "_b200_probe": ["tma_probe.cu", "tmap.cpp", "probe_bind.cpp"],   # hardware probe, not on any hot path
-    "_b200_ops": ["elementwise.cu", "head_stem.cu", "mobilenet.cu", "optim.cu", "mobilenet_bwd.cu", "ops_bind.cpp"],
+    "_b200_ops": ["elementwise.cu", "head_stem.cu", "mobilenet.cu", "optim.cu", "mobilenet_bwd.cu", "augment.cu",
+                  "ops_bind.cpp"],
     "_b200_comm": ["allreduce.cu", "comm_bind.cpp"],
     "_b200_loader": ["ring_loader.cpp"],
     "_b200_jpeg": ["jpeg_decode.cpp", "jpeg_resize.cu"],   # nvJPEG (library) decode + our batched resize kernel
@@ -48,7 +49,7 @@ LDFLAGS: Dict[str, List[str]] = {
 HEADERS: Dict[str, List[str]] = {
     "_b200_conv": ["ptx.cuh", "conv_igemm.cuh", "conv_params.h", "conv_api.h"],
     "_b200_probe": ["ptx.cuh", "conv_params.h", "conv_api.h"],
-    "_b200_ops": ["ops_api.h"],
+    "_b200_ops": ["ops_api.h", "hash.cuh"],
     "_b200_comm": ["comm_api.h"],
     "_b200_loader": [],
     "_b200_jpeg": [],

@@ -51,13 +51,12 @@ class FlatOptimizer:
         if params.is_cuda:
             from .. import ops
 
+            from ..utils.pinned import PinnedUpload
+
             self._ext = ops.ext("_b200_ops")
-            # ring of pinned staging rows: the host runs several steps ahead of the device, so the row an async copy
-            # reads from must not be refilled before that copy has executed (depth >> steps in flight)
-            self._hyper_ring = torch.zeros(64, 8, dtype=torch.float32).pin_memory()
-            self._hyper_events = [None] * 64
-            self._hyper_slot = 0
-            self._hyper_host = self._hyper_ring[0]
+            # ring of pinned staging rows: the host runs several steps ahead of the device (depth >> steps in flight)
+            self._hyper_upload = PinnedUpload(self._hyper)
+            self._hyper_host = self._hyper_upload.ring[0]
         else:
             self._hyper_host = torch.zeros(8, dtype=torch.float32)
         self.push_hyper()
@@ -78,22 +77,12 @@ class FlatOptimizer:
 
     def push_hyper(self) -> None:
         """Host -> device copy of the 8 hyper-parameters (outside any CUDA graph)."""
-        ring = getattr(self, "_hyper_ring", None)
-        if ring is None:
+        upload = getattr(self, "_hyper_upload", None)
+        if upload is None:
             self._fill_hyper(self._hyper_host)
             self._hyper.copy_(self._hyper_host, non_blocking=True)
             return
-        i = self._hyper_slot
-        self._hyper_slot = (i + 1) % ring.shape[0]
-        ev = self._hyper_events[i]
-        if ev is not None:
-            ev.synchronize()  # the copy that last read this row has executed (64 steps ago: never waits in practice)
-        self._hyper_host = ring[i]
-        self._fill_hyper(self._hyper_host)
-        self._hyper.copy_(self._hyper_host, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._hyper_events[i] = ev
+        self._hyper_host = upload.push(self._fill_hyper)
 
     def begin_step(self) -> None:
         """Advance the step counter and refresh the device hyper-parameters; call before (re)playing a step."""

@@ -9,10 +9,16 @@ from typing import Optional
 import torch
 
 
+def _augmentation(model) -> Optional[dict]:
+    aug = getattr(model, "augmentation", None)
+    return aug.to_dict() if aug is not None else None
+
+
 def _describe(model) -> dict:
     if hasattr(model, "param_specs"):  # native engines (ResNet50Engine, MobileNetV2Engine)
         desc = {"arch": getattr(model, "arch", "resnet50"), "num_classes": model.num_classes, "image_size": model.image_size,
-                "dropout": model.dropout, "batch": model.batch, "engine": True}
+                "dropout": model.dropout, "batch": model.batch, "engine": True, "augmentation": _augmentation(model),
+                "seed": model.seed}   # the seed keys the augmentation draws: a reloaded engine continues the sequence
         if desc["arch"] == "mobilenetv2":
             desc["fine_tune_at"] = model.fine_tune_at
         return desc
@@ -20,7 +26,8 @@ def _describe(model) -> dict:
 
     if isinstance(model, FrozenBaseClassifier):
         return {"arch": "mobilenetv2", "num_classes": model.fc.out_features, "dropout": model.dropout.p,
-                "freeze_base": model.freeze_base, "fine_tune_at": model.fine_tune_at}
+                "freeze_base": model.freeze_base, "fine_tune_at": model.fine_tune_at,
+                "augmentation": _augmentation(model), "augmentation_seed": model.augmentation_seed}
     return {"arch": "pickle"}
 
 
@@ -51,7 +58,7 @@ def log_model(model_or_trainer, artifact_path: str = "model") -> str:
 def load_model(model_uri: str, batch_size: Optional[int] = None, device=None):
     """Returns a compiled-for-inference `Trainer` (has `.predict`, `.summary`, `.model`)."""
     from . import resolve_uri
-    from ..models import build_model
+    from ..models import Augmentation, build_model
     from ..train import Trainer
 
     path = resolve_uri(model_uri)
@@ -64,21 +71,24 @@ def load_model(model_uri: str, batch_size: Optional[int] = None, device=None):
             model = cloudpickle.load(f)
         return Trainer(model, device=device)
     sd = torch.load(os.path.join(path, "weights.pt"), map_location="cpu")
+    aug = Augmentation.from_dict(desc.get("augmentation"))
     if desc["arch"] == "resnet50":
         if torch.cuda.is_available():
             model = build_model(desc["image_size"], desc["image_size"], 3, desc["num_classes"], desc["dropout"],
-                                arch="resnet50", batch_size=batch_size or desc["batch"], device=device)
+                                arch="resnet50", batch_size=batch_size or desc["batch"], device=device, augmentation=aug,
+                                seed=desc.get("seed", 0))
             model.load_state_dict(sd)
-        else:  # CPU box: same weights in the torchvision-architecture module
+        else:  # CPU box: same weights in the torchvision-architecture module (inference only: no augmentation)
             model = build_model(num_classes=desc["num_classes"], arch="resnet50_torch")
             model.load_state_dict(sd, strict=False)
     elif desc.get("engine") and torch.cuda.is_available():  # saved from the native MobileNetV2 engine
         model = build_model(desc["image_size"], desc["image_size"], 3, desc["num_classes"], desc["dropout"],
                             arch="mobilenetv2", batch_size=batch_size or desc["batch"], device=device,
-                            fine_tune_at=desc.get("fine_tune_at"))
+                            fine_tune_at=desc.get("fine_tune_at"), augmentation=aug, seed=desc.get("seed", 0))
         model.load_state_dict(sd)
     else:
         model = build_model(num_classes=desc["num_classes"], dropout=desc["dropout"], arch="mobilenetv2_torch",
-                            freeze_base=desc.get("freeze_base", True), fine_tune_at=desc.get("fine_tune_at"))
+                            freeze_base=desc.get("freeze_base", True), fine_tune_at=desc.get("fine_tune_at"),
+                            augmentation=aug, seed=desc.get("augmentation_seed", 0))
         model.load_state_dict(sd)
     return Trainer(model, device=device)

@@ -185,10 +185,24 @@ class _ModuleBackend:
         x = torch.as_tensor(x).to(self.device, non_blocking=True)
         return self.preprocess(x)
 
+    def _augmented(self, x) -> torch.Tensor:
+        """The uint8 NHWC batch warped by ``module.augmentation`` at the optimizer's current step (the reference
+        implementation of the engines' augmentation kernels, same draws for the same seed, rank and step)."""
+        from ..models.augment import augment_key, augment_reference
+
+        x = torch.as_tensor(x)
+        if x.dtype != torch.uint8:
+            raise ValueError(f"augmentation needs the uint8 [N, H, W, 3] batch, got {x.dtype}")
+        opt = self.optimizer.opt if hasattr(self.optimizer, "opt") else self.optimizer
+        key = augment_key(getattr(self.module, "augmentation_seed", 0), dist_core.rank())
+        return augment_reference(self.module.augmentation, x.to(self.device, non_blocking=True), key, opt.t)
+
     def train_batch(self, x, y) -> None:
         self.module.train()
         y = torch.as_tensor(y).to(self.device, non_blocking=True)
         self.optimizer.begin_step()
+        if getattr(self.module, "augmentation", None) is not None:
+            x = self._augmented(x)
         self.flat.zero_grad()
         if self._dist:
             self.optimizer.start_backward()
