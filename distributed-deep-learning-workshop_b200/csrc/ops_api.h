@@ -77,12 +77,43 @@ void weight_prep_batched(const float* params, void* wd, const int64_t* table, in
 
 // Fused flat-buffer optimizers.  `hyper` is a DEVICE array (so LR schedules do not invalidate CUDA graphs):
 //   [0] lr  [1] momentum/beta1  [2] beta2/rho  [3] eps  [4] weight_decay  [5] grad_scale  [6] bias_corr1  [7] bias_corr2
+//   [8] clip threshold  [9] the host's grad_scale  [10..15] unused
+// The update kernels read slots 0-7 only (their bindings accept >= kHyperLen); the clip and LAMB passes need all
+// kHyperSlots.  The global-norm clip writes [5] = [9] * factor, so repeating a step never compounds the factor.
 constexpr int kHyperLen = 8;
+constexpr int kHyperSlots = 16;
+constexpr int kHypClip = 8;
+constexpr int kHypGradScale = 9;
 void sgd_step(float* p, const float* g, float* mom, void* p16, int64_t n, const float* hyper, bool nesterov,
               cudaStream_t s);
 void adam_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper, cudaStream_t s);
 void adadelta_step(float* p, const float* g, float* sq, float* acc, void* p16, int64_t n, const float* hyper,
                    cudaStream_t s);
+void adamw_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper, cudaStream_t s);
+// mom / avg: nullptr without momentum / when not centered
+void rmsprop_step(float* p, const float* g, float* sq, float* mom, float* avg, void* p16, int64_t n,
+                  const float* hyper, cudaStream_t s);
+void adagrad_step(float* p, const float* g, float* acc, void* p16, int64_t n, const float* hyper, cudaStream_t s);
+void adamax_step(float* p, const float* g, float* m, float* u, void* p16, int64_t n, const float* hyper,
+                 cudaStream_t s);
+// Chunk table: int64 [nchunks, kChunkFields] = (lo, hi, segment), lo / hi multiples of 4, hi - lo <= kChunkMax.
+// Segment table: int64 [nseg, 2] = (first chunk, end chunk).  partial: fp32 [nchunks] (x2 for LAMB);
+// sums: fp32 [2, nseg + 1] (per-segment sums of squares, then the total); factor: fp32 [nseg].
+constexpr int kChunkFields = 3;
+constexpr int64_t kChunkMax = 8192;
+constexpr int kMaxSegments = 1 << 20;
+enum : int { kFinSums = 0, kFinClipGlobal = 1, kFinClipNorm = 2, kFinLamb = 3 };
+void segment_sumsq(const float* g, int64_t n, const int64_t* chunks, int64_t nchunks, float* partial,
+                   const float* hyper, cudaStream_t s);
+void segment_finalize(const float* partial, int64_t nchunks, const int64_t* segs, int nseg, float* sums,
+                      float* factor, float* hyper, int mode, cudaStream_t s);
+// factor != nullptr: clipnorm (g *= grad_scale * factor[segment]); nullptr: clipvalue (clamp(g * grad_scale, -c, c))
+void clip_apply(float* g, int64_t n, const int64_t* chunks, int64_t nchunks, const float* factor, int nseg,
+                const float* hyper, cudaStream_t s);
+void lamb_moments(const float* p, const float* g, float* m, float* v, int64_t n, const int64_t* chunks,
+                  int64_t nchunks, float* partial, const float* hyper, cudaStream_t s);
+void lamb_apply(float* p, const float* m, const float* v, void* p16, int64_t n, const int64_t* chunks,
+                int64_t nchunks, const float* phi, int nseg, const float* hyper, cudaStream_t s);
 void cast_f32_to_bf16(const float* x, void* out, int64_t n, cudaStream_t s);
 
 // MobileNetV2 fine-tuning backward with inference-mode BatchNorm (csrc/mobilenet_bwd.cu).

@@ -443,6 +443,119 @@ void adadelta_step(Tensor p, Tensor g, Tensor sq, Tensor acc, OptT p16, Tensor h
                       p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
   after();
 }
+void adamw_step(Tensor p, Tensor g, Tensor m, Tensor v, OptT p16, Tensor hyper) {
+  optim_operands(p, {{&g, "g"}, {&m, "m"}, {&v, "v"}}, p16, hyper);
+  b200::adamw_step(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
+                   p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
+  after();
+}
+void rmsprop_step(Tensor p, Tensor g, Tensor sq, OptT mom, OptT avg, OptT p16, Tensor hyper) {
+  optim_operands(p, {{&g, "g"}, {&sq, "sq"}}, p16, hyper);
+  if (mom.has_value()) vec(*mom, at::kFloat, p.numel(), "mom");
+  if (avg.has_value()) vec(*avg, at::kFloat, p.numel(), "avg");
+  b200::rmsprop_step(p.data_ptr<float>(), g.data_ptr<float>(), sq.data_ptr<float>(),
+                     mom.has_value() ? mom->data_ptr<float>() : nullptr, avg.has_value() ? avg->data_ptr<float>() : nullptr,
+                     p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
+  after();
+}
+void adagrad_step(Tensor p, Tensor g, Tensor acc, OptT p16, Tensor hyper) {
+  optim_operands(p, {{&g, "g"}, {&acc, "acc"}}, p16, hyper);
+  b200::adagrad_step(p.data_ptr<float>(), g.data_ptr<float>(), acc.data_ptr<float>(),
+                     p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
+  after();
+}
+void adamax_step(Tensor p, Tensor g, Tensor m, Tensor u, OptT p16, Tensor hyper) {
+  optim_operands(p, {{&g, "g"}, {&m, "m"}, {&u, "u"}}, p16, hyper);
+  b200::adamax_step(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), u.data_ptr<float>(),
+                    p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
+  after();
+}
+
+// ---- chunked clip / LAMB passes: flat buffer x (fp32, n % 4 == 0, 16-byte aligned), chunk table, 16-slot hyper array
+static int64_t chunk_operands(const Tensor& x, const Tensor& chunks, const Tensor& hyper) {
+  chk(x, at::kFloat, "flat buffer");
+  TORCH_CHECK(x.numel() % 4 == 0, "flat buffer: element count must be a multiple of 4");
+  aligned(x, 16, "flat buffer");
+  chk(chunks, at::kLong, "chunks");
+  TORCH_CHECK(chunks.dim() == 2 && chunks.size(1) == b200::kChunkFields && chunks.size(0) >= 1 &&
+              chunks.size(0) < (int64_t(1) << 31), "chunks: int64 [nchunks (1 .. 2^31 - 1), 3] = (lo, hi, segment)");
+  vec(hyper, at::kFloat, hyper.numel(), "hyper", 4);
+  TORCH_CHECK(hyper.numel() >= b200::kHyperSlots, "hyper must hold 16 values for the clip and LAMB passes");
+  TORCH_CHECK(chunks.device() == x.device() && hyper.device() == x.device(),
+              "chunks and hyper must be on the device of the flat buffer");
+  return chunks.size(0);
+}
+static void partial_operand(const Tensor& partial, int64_t rows, int64_t nchunks, const Tensor& like) {
+  vec(partial, at::kFloat, rows * nchunks, "partial", 4);
+  TORCH_CHECK(partial.dim() == (rows == 1 ? 1 : 2), "partial: fp32 [nchunks], or [2, nchunks] for LAMB");
+  TORCH_CHECK(partial.device() == like.device(), "partial must be on the device of the flat buffer");
+}
+void segment_sumsq(Tensor g, Tensor chunks, Tensor partial, Tensor hyper) {
+  const int64_t nc = chunk_operands(g, chunks, hyper);
+  partial_operand(partial, 1, nc, g);
+  b200::segment_sumsq(g.data_ptr<float>(), g.numel(), chunks.data_ptr<int64_t>(), nc, partial.data_ptr<float>(),
+                      hyper.data_ptr<float>(), cur());
+  after();
+}
+void segment_finalize(Tensor partial, Tensor segs, Tensor sums, Tensor factor, Tensor hyper, int64_t mode) {
+  TORCH_CHECK(mode >= b200::kFinSums && mode <= b200::kFinLamb, "mode: 0 sums, 1 global clip, 2 per-segment clip, 3 LAMB");
+  const int64_t rows = mode == b200::kFinLamb ? 2 : 1;
+  TORCH_CHECK(partial.dim() == (rows == 1 ? 1 : 2) && (rows == 1 || partial.size(0) == 2),
+              "partial: fp32 [nchunks], or [2, nchunks] for LAMB");
+  const int64_t nc = partial.size(-1);
+  partial_operand(partial, rows, nc, partial);
+  chk(segs, at::kLong, "segs");
+  TORCH_CHECK(segs.dim() == 2 && segs.size(1) == 2 && segs.size(0) >= 1 && segs.size(0) <= b200::kMaxSegments,
+              "segs: int64 [nseg (1 .. 2^20), 2] = (first chunk, end chunk)");
+  const int64_t ns = segs.size(0);
+  vec(sums, at::kFloat, 2 * (ns + 1), "sums", 4);
+  vec(factor, at::kFloat, ns, "factor", 4);
+  vec(hyper, at::kFloat, hyper.numel(), "hyper", 4);
+  TORCH_CHECK(hyper.numel() >= b200::kHyperSlots, "hyper must hold 16 values for the clip and LAMB passes");
+  for (const Tensor* t : {&segs, &sums, &factor, &hyper})
+    TORCH_CHECK(t->device() == partial.device(), "segs, sums, factor and hyper must be on the device of partial");
+  b200::segment_finalize(partial.data_ptr<float>(), nc, segs.data_ptr<int64_t>(), (int)ns, sums.data_ptr<float>(),
+                         factor.data_ptr<float>(), hyper.data_ptr<float>(), (int)mode, cur());
+  after();
+}
+void clip_apply(Tensor g, Tensor chunks, OptT factor, Tensor hyper) {
+  const int64_t nc = chunk_operands(g, chunks, hyper);
+  if (factor.has_value()) {
+    chk(*factor, at::kFloat, "factor");
+    TORCH_CHECK(factor->dim() == 1 && factor->numel() >= 1 && factor->numel() <= b200::kMaxSegments &&
+                factor->device() == g.device(),
+                "factor: fp32 [nseg] on the device of g");
+  }
+  b200::clip_apply(g.data_ptr<float>(), g.numel(), chunks.data_ptr<int64_t>(), nc, fp(factor),
+                   factor.has_value() ? (int)factor->numel() : 0, hyper.data_ptr<float>(), cur());
+  after();
+}
+void lamb_moments(Tensor p, Tensor g, Tensor m, Tensor v, Tensor chunks, Tensor partial, Tensor hyper) {
+  const int64_t nc = chunk_operands(p, chunks, hyper);
+  for (const auto& [t, name] : {std::pair<const Tensor*, const char*>{&g, "g"}, {&m, "m"}, {&v, "v"}}) {
+    vec(*t, at::kFloat, p.numel(), name);
+    TORCH_CHECK(t->device() == p.device(), name, " must be on the device of p");
+  }
+  partial_operand(partial, 2, nc, p);
+  b200::lamb_moments(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(), p.numel(),
+                     chunks.data_ptr<int64_t>(), nc, partial.data_ptr<float>(), hyper.data_ptr<float>(), cur());
+  after();
+}
+void lamb_apply(Tensor p, Tensor m, Tensor v, OptT p16, Tensor chunks, Tensor phi, Tensor hyper) {
+  const int64_t nc = chunk_operands(p, chunks, hyper);
+  for (const auto& [t, name] : {std::pair<const Tensor*, const char*>{&m, "m"}, {&v, "v"}}) {
+    vec(*t, at::kFloat, p.numel(), name);
+    TORCH_CHECK(t->device() == p.device(), name, " must be on the device of p");
+  }
+  if (p16.has_value()) vec(*p16, at::kBFloat16, p.numel(), "p16", 8);
+  chk(phi, at::kFloat, "phi");
+  TORCH_CHECK(phi.dim() == 1 && phi.numel() >= 1 && phi.numel() <= b200::kMaxSegments && phi.device() == p.device(),
+              "phi: fp32 [nseg] on the device of p");
+  b200::lamb_apply(p.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
+                   p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), chunks.data_ptr<int64_t>(), nc,
+                   phi.data_ptr<float>(), (int)phi.numel(), hyper.data_ptr<float>(), cur());
+  after();
+}
 void cast_bf16(Tensor x, Tensor out) {
   chk(x, at::kFloat, "x");
   TORCH_CHECK(x.numel() % 4 == 0, "x: element count must be a multiple of 4");
@@ -621,6 +734,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sgd_step", &sgd_step);
   m.def("adam_step", &adam_step);
   m.def("adadelta_step", &adadelta_step);
+  m.def("adamw_step", &adamw_step);
+  m.def("rmsprop_step", &rmsprop_step, py::arg("p"), py::arg("g"), py::arg("sq"), py::arg("mom"), py::arg("avg"),
+        py::arg("p16"), py::arg("hyper"));
+  m.def("adagrad_step", &adagrad_step);
+  m.def("adamax_step", &adamax_step);
+  m.def("segment_sumsq", &segment_sumsq);
+  m.def("segment_finalize", &segment_finalize);
+  m.def("clip_apply", &clip_apply);
+  m.def("lamb_moments", &lamb_moments);
+  m.def("lamb_apply", &lamb_apply);
   m.def("cast_bf16", &cast_bf16);
   m.def("launch_count", [] { return g_launches; });
   m.def("reset_launch_count", [] { g_launches = 0; });

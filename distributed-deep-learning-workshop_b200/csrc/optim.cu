@@ -39,6 +39,8 @@ __global__ void sgd_kernel(float* __restrict__ p, const float* __restrict__ g, f
   }
 }
 
+// DECOUPLED (AdamW): p *= 1 - lr * wd before the Adam step, and the gradient carries no L2 term.
+template <bool DECOUPLED>
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m1,
                             float* __restrict__ v1, __nv_bfloat16* __restrict__ p16, int64_t n4,
                             const float* __restrict__ hyper) {
@@ -46,6 +48,7 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
   const float bc1 = hyper[6], bc2 = hyper[7];
   const float step = lr / bc1;
   const float inv_sqrt_bc2 = rsqrtf(bc2);
+  const float decay = 1.f - lr * wd;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     float4 w = reinterpret_cast<float4*>(p)[i];
     float4 gr = reinterpret_cast<const float4*>(g)[i];
@@ -54,7 +57,13 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     float* wf = &w.x; float* gf = &gr.x; float* mf = &m.x; float* vf = &v.x;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float d = fmaf(wd, wf[k], gf[k] * gs);
+      float d;
+      if constexpr (DECOUPLED) {
+        wf[k] *= decay;
+        d = gf[k] * gs;
+      } else {
+        d = fmaf(wd, wf[k], gf[k] * gs);
+      }
       mf[k] = fmaf(b1, mf[k], (1.f - b1) * d);
       vf[k] = fmaf(b2, vf[k], (1.f - b2) * d * d);
       const float denom = sqrtf(vf[k]) * inv_sqrt_bc2 + eps;
@@ -92,6 +101,310 @@ __global__ void adadelta_kernel(float* __restrict__ p, const float* __restrict__
   }
 }
 
+// torch.optim.RMSprop: v = rho v + (1 - rho) d^2; CENTERED: a = rho a + (1 - rho) d, denom = sqrt(v - a^2) + eps
+// (v - a^2 >= 0 in exact arithmetic; clamped at 0 so that rounding cannot make it NaN); MOMENTUM: buf = mu buf + d / denom,
+// p -= lr buf; otherwise p -= lr d / denom.
+template <bool CENTERED, bool MOMENTUM>
+__global__ void rmsprop_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq,
+                               float* __restrict__ mom, float* __restrict__ avg, __nv_bfloat16* __restrict__ p16,
+                               int64_t n4, const float* __restrict__ hyper) {
+  const float lr = hyper[0], mu = hyper[1], rho = hyper[2], eps = hyper[3], wd = hyper[4], gs = hyper[5];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 w = reinterpret_cast<float4*>(p)[i];
+    float4 gr = reinterpret_cast<const float4*>(g)[i];
+    float4 s = reinterpret_cast<float4*>(sq)[i];
+    float4 b = MOMENTUM ? reinterpret_cast<float4*>(mom)[i] : float4{};
+    float4 a = CENTERED ? reinterpret_cast<float4*>(avg)[i] : float4{};
+    float* wf = &w.x; float* gf = &gr.x; float* sf = &s.x; float* bf = &b.x; float* af = &a.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float d = fmaf(wd, wf[k], gf[k] * gs);
+      sf[k] = fmaf(rho, sf[k], (1.f - rho) * d * d);
+      float var = sf[k];
+      if constexpr (CENTERED) {
+        af[k] = fmaf(rho, af[k], (1.f - rho) * d);
+        var = fmaxf(fmaf(-af[k], af[k], sf[k]), 0.f);
+      }
+      const float q = d / (sqrtf(var) + eps);
+      if constexpr (MOMENTUM) {
+        bf[k] = fmaf(mu, bf[k], q);
+        wf[k] = fmaf(-lr, bf[k], wf[k]);
+      } else {
+        wf[k] = fmaf(-lr, q, wf[k]);
+      }
+    }
+    reinterpret_cast<float4*>(p)[i] = w;
+    reinterpret_cast<float4*>(sq)[i] = s;
+    if (MOMENTUM) reinterpret_cast<float4*>(mom)[i] = b;
+    if (CENTERED) reinterpret_cast<float4*>(avg)[i] = a;
+    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
+  }
+}
+
+// torch.optim.Adagrad (lr_decay 0): acc += d^2, p -= lr d / (sqrt(acc) + eps).
+__global__ void adagrad_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ acc,
+                               __nv_bfloat16* __restrict__ p16, int64_t n4, const float* __restrict__ hyper) {
+  const float lr = hyper[0], eps = hyper[3], wd = hyper[4], gs = hyper[5];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 w = reinterpret_cast<float4*>(p)[i];
+    float4 gr = reinterpret_cast<const float4*>(g)[i];
+    float4 a = reinterpret_cast<float4*>(acc)[i];
+    float* wf = &w.x; float* gf = &gr.x; float* af = &a.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float d = fmaf(wd, wf[k], gf[k] * gs);
+      af[k] = fmaf(d, d, af[k]);
+      wf[k] = fmaf(-lr, d / (sqrtf(af[k]) + eps), wf[k]);
+    }
+    reinterpret_cast<float4*>(p)[i] = w;
+    reinterpret_cast<float4*>(acc)[i] = a;
+    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
+  }
+}
+
+// torch.optim.Adamax: m = b1 m + (1 - b1) d, u = max(b2 u, |d| + eps), p -= (lr / bc1) m / u.
+__global__ void adamax_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m1,
+                              float* __restrict__ u1, __nv_bfloat16* __restrict__ p16, int64_t n4,
+                              const float* __restrict__ hyper) {
+  const float lr = hyper[0], b1 = hyper[1], b2 = hyper[2], eps = hyper[3], wd = hyper[4], gs = hyper[5];
+  const float step = lr / hyper[6];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 w = reinterpret_cast<float4*>(p)[i];
+    float4 gr = reinterpret_cast<const float4*>(g)[i];
+    float4 m = reinterpret_cast<float4*>(m1)[i];
+    float4 u = reinterpret_cast<float4*>(u1)[i];
+    float* wf = &w.x; float* gf = &gr.x; float* mf = &m.x; float* uf = &u.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float d = fmaf(wd, wf[k], gf[k] * gs);
+      mf[k] = fmaf(b1, mf[k], (1.f - b1) * d);
+      uf[k] = fmaxf(b2 * uf[k], fabsf(d) + eps);
+      wf[k] = wf[k] - step * mf[k] / uf[k];
+    }
+    reinterpret_cast<float4*>(p)[i] = w;
+    reinterpret_cast<float4*>(m1)[i] = m;
+    reinterpret_cast<float4*>(u1)[i] = u;
+    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ chunked passes
+// The clip and LAMB passes work on a chunk table (kChunkFields int64 per row: lo, hi, segment): every segment (one
+// parameter tensor) of the flat buffer is cut into chunks of at most kChunkMax floats, float4-aligned, and no chunk spans
+// two segments.  One CTA handles one chunk, so a per-segment value (clip factor, LAMB trust ratio) is one load per CTA,
+// and a chunk's sum of squares is reduced in a fixed order into one partial: no atomics, bit-reproducible.
+constexpr int kChunkThreads = 256;
+
+struct Chunk {
+  int64_t lo4, hi4;
+  int seg;
+};
+// rows outside [0, n) or not float4-aligned are skipped (the host builds and checks the table; this only keeps a bad
+// row from touching memory it does not own)
+__device__ __forceinline__ bool load_chunk(const int64_t* __restrict__ chunks, int64_t n, Chunk& c,
+                                           int64_t nseg = INT32_MAX) {
+  const int64_t* row = chunks + (int64_t)blockIdx.x * kChunkFields;
+  const int64_t lo = row[0], hi = row[1];
+  c.lo4 = lo >> 2;
+  c.hi4 = hi >> 2;
+  c.seg = (int)row[2];
+  return lo >= 0 && lo <= hi && hi <= n && ((lo | hi) & 3) == 0 && hi - lo <= kChunkMax && row[2] >= 0 &&
+         row[2] < nseg;
+}
+
+// fixed-order CTA sum of one value per thread (kChunkThreads threads): warp trees, then warp 0 over the warp sums
+__device__ __forceinline__ float block_sum(float x, float* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) red[warp] = x;
+  __syncthreads();
+  x = lane < kChunkThreads / 32 ? red[lane] : 0.f;
+  if (warp == 0) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
+  }
+  return x;   // valid in thread 0
+}
+
+// partial[chunk] = sum over the chunk of (g * hyper[kHypGradScale])^2
+__global__ void __launch_bounds__(kChunkThreads) segment_sumsq_kernel(const float* __restrict__ g, int64_t n,
+                                                                      const int64_t* __restrict__ chunks,
+                                                                      float* __restrict__ partial,
+                                                                      const float* __restrict__ hyper) {
+  __shared__ float red[kChunkThreads / 32];
+  Chunk c;
+  const bool ok = load_chunk(chunks, n, c);
+  const float gs = hyper[kHypGradScale];
+  float acc = 0.f;
+  if (ok) {
+    for (int64_t i = c.lo4 + threadIdx.x; i < c.hi4; i += kChunkThreads) {
+      const float4 v = reinterpret_cast<const float4*>(g)[i];
+      const float x0 = v.x * gs, x1 = v.y * gs, x2 = v.z * gs, x3 = v.w * gs;
+      acc = fmaf(x0, x0, acc);
+      acc = fmaf(x1, x1, acc);
+      acc = fmaf(x2, x2, acc);
+      acc = fmaf(x3, x3, acc);
+    }
+  }
+  acc = block_sum(acc, red);
+  if (threadIdx.x == 0) partial[blockIdx.x] = acc;
+}
+
+// One CTA of 32 warps.  Segment s's partials (chunks segs[s].first .. segs[s].end) are summed by one warp: lane l adds
+// chunks first + l, first + l + 32, ... in order, then a shuffle tree; the global sum is the same warp reduction over
+// the segment sums in segment order.  sums[k * (nseg + 1) + s] (k = 0: partial_a, 1: partial_b), global at index nseg.
+// mode kFinClipGlobal: hyper[GSCALE] = hyper[kHypGradScale] * c / max(norm, c) with c = hyper[kHypClip]
+// mode kFinClipNorm:   factor[s] = c / max(norm_s, c)
+// (the clip factor is exactly 1 when the norm does not exceed c)
+// mode kFinLamb:       factor[s] = norm(p)_s / norm(r)_s, or 1 when either is 0 (partial_a: p^2, partial_b: r^2)
+constexpr int kFinThreads = 1024;
+// Keras's c / max(norm, c), written so that a norm within the threshold gives exactly 1 (an approximate c / c need not)
+__device__ __forceinline__ float clip_factor(float sumsq, float c) {
+  const float norm = sqrtf(sumsq);
+  return norm > c ? c / norm : 1.f;
+}
+__device__ __forceinline__ float warp_sum_strided(const float* __restrict__ x, int64_t first, int64_t end) {
+  const int lane = threadIdx.x & 31;
+  float acc = 0.f;
+  for (int64_t j = first + lane; j < end; j += 32) acc += x[j];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
+  return __shfl_sync(0xffffffffu, acc, 0);
+}
+__global__ void __launch_bounds__(kFinThreads) segment_finalize_kernel(const float* __restrict__ partial,
+                                                                       int64_t nchunks,
+                                                                       const int64_t* __restrict__ segs, int nseg,
+                                                                       float* __restrict__ sums,
+                                                                       float* __restrict__ factor,
+                                                                       float* __restrict__ hyper, int mode) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nk = mode == kFinLamb ? 2 : 1;
+  const float c = hyper[kHypClip];
+  for (int s = warp; s < nseg; s += kFinThreads / 32) {
+    const int64_t first = max(segs[2 * s], (int64_t)0), end = min(segs[2 * s + 1], nchunks);   // bad rows: no reads
+    float sk[2];
+    for (int k = 0; k < nk; ++k) {
+      sk[k] = warp_sum_strided(partial + k * nchunks, first, end);
+      if (lane == 0) sums[k * (nseg + 1) + s] = sk[k];
+    }
+    if (lane == 0) {
+      if (mode == kFinClipNorm) {
+        factor[s] = clip_factor(sk[0], c);
+      } else if (mode == kFinLamb) {
+        const float pn = sqrtf(sk[0]), rn = sqrtf(sk[1]);
+        factor[s] = (pn > 0.f && rn > 0.f) ? pn / rn : 1.f;
+      }
+    }
+  }
+  __syncthreads();
+  if (warp == 0) {
+    for (int k = 0; k < nk; ++k) {
+      const float tot = warp_sum_strided(sums + k * (nseg + 1), 0, nseg);
+      if (lane == 0) sums[k * (nseg + 1) + nseg] = tot;
+      if (k == 0 && lane == 0 && mode == kFinClipGlobal)
+        hyper[5] = hyper[kHypGradScale] * clip_factor(tot, c);
+    }
+  }
+}
+
+// clipnorm (factor != nullptr): g = g * gs * factor[segment]; clipvalue: g = clamp(g * gs, -c, c)
+__global__ void __launch_bounds__(kChunkThreads) clip_apply_kernel(float* __restrict__ g, int64_t n,
+                                                                   const int64_t* __restrict__ chunks,
+                                                                   const float* __restrict__ factor, int nseg,
+                                                                   const float* __restrict__ hyper) {
+  Chunk c;
+  if (!load_chunk(chunks, n, c, factor != nullptr ? nseg : INT32_MAX)) return;
+  const float gs = hyper[kHypGradScale], lim = hyper[kHypClip];
+  const float f = factor != nullptr ? gs * factor[c.seg] : gs;
+  for (int64_t i = c.lo4 + threadIdx.x; i < c.hi4; i += kChunkThreads) {
+    float4 v = reinterpret_cast<float4*>(g)[i];
+    float* vf = &v.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) vf[k] = factor != nullptr ? vf[k] * f : fminf(fmaxf(vf[k] * f, -lim), lim);
+    reinterpret_cast<float4*>(g)[i] = v;
+  }
+}
+
+// LAMB (You et al. 2019) direction r = m_hat / (sqrt(v_hat) + eps) + wd p, written with explicit intrinsics so that
+// pass 1 (norms) and pass 3 (update) evaluate the same instruction sequence on the same stored m, v, p.
+__device__ __forceinline__ float lamb_dir(float m, float v, float w, float inv_bc1, float inv_sqrt_bc2, float eps,
+                                          float wd) {
+  const float denom = __fmaf_rn(sqrtf(v), inv_sqrt_bc2, eps);
+  return __fmaf_rn(wd, w, __fdividef(__fmul_rn(m, inv_bc1), denom));
+}
+struct LambHyper {
+  float b1, b2, eps, wd, gs, inv_bc1, inv_sqrt_bc2;
+  __device__ explicit LambHyper(const float* __restrict__ h)
+      : b1(h[1]), b2(h[2]), eps(h[3]), wd(h[4]), gs(h[5]), inv_bc1(1.f / h[6]), inv_sqrt_bc2(rsqrtf(h[7])) {}
+};
+
+// pass 1: m, v update; partial[chunk] = sum p^2, partial[nchunks + chunk] = sum r^2
+__global__ void __launch_bounds__(kChunkThreads) lamb_moments_kernel(const float* __restrict__ p,
+                                                                     const float* __restrict__ g, float* __restrict__ m1,
+                                                                     float* __restrict__ v1, int64_t n,
+                                                                     const int64_t* __restrict__ chunks,
+                                                                     int64_t nchunks, float* __restrict__ partial,
+                                                                     const float* __restrict__ hyper) {
+  __shared__ float red[kChunkThreads / 32];
+  Chunk c;
+  const bool ok = load_chunk(chunks, n, c);
+  const LambHyper h(hyper);
+  float pp = 0.f, rr = 0.f;
+  if (ok) {
+    for (int64_t i = c.lo4 + threadIdx.x; i < c.hi4; i += kChunkThreads) {
+      const float4 w = reinterpret_cast<const float4*>(p)[i];
+      const float4 gr = reinterpret_cast<const float4*>(g)[i];
+      float4 m = reinterpret_cast<float4*>(m1)[i];
+      float4 v = reinterpret_cast<float4*>(v1)[i];
+      const float* wf = &w.x; const float* gf = &gr.x; float* mf = &m.x; float* vf = &v.x;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float d = gf[k] * h.gs;
+        mf[k] = fmaf(h.b1, mf[k], (1.f - h.b1) * d);
+        vf[k] = fmaf(h.b2, vf[k], (1.f - h.b2) * d * d);
+        const float r = lamb_dir(mf[k], vf[k], wf[k], h.inv_bc1, h.inv_sqrt_bc2, h.eps, h.wd);
+        pp = fmaf(wf[k], wf[k], pp);
+        rr = fmaf(r, r, rr);
+      }
+      reinterpret_cast<float4*>(m1)[i] = m;
+      reinterpret_cast<float4*>(v1)[i] = v;
+    }
+  }
+  pp = block_sum(pp, red);
+  __syncthreads();   // red is reused
+  rr = block_sum(rr, red);
+  if (threadIdx.x == 0) {
+    partial[blockIdx.x] = pp;
+    partial[nchunks + blockIdx.x] = rr;
+  }
+}
+
+// pass 3: p -= lr * phi[segment] * r, bf16 copy in the same pass
+__global__ void __launch_bounds__(kChunkThreads) lamb_apply_kernel(float* __restrict__ p,
+                                                                   const float* __restrict__ m1,
+                                                                   const float* __restrict__ v1,
+                                                                   __nv_bfloat16* __restrict__ p16, int64_t n,
+                                                                   const int64_t* __restrict__ chunks,
+                                                                   const float* __restrict__ phi, int nseg,
+                                                                   const float* __restrict__ hyper) {
+  Chunk c;
+  if (!load_chunk(chunks, n, c, nseg)) return;
+  const LambHyper h(hyper);
+  const float step = -hyper[0] * phi[c.seg];
+  for (int64_t i = c.lo4 + threadIdx.x; i < c.hi4; i += kChunkThreads) {
+    float4 w = reinterpret_cast<float4*>(p)[i];
+    const float4 m = reinterpret_cast<const float4*>(m1)[i];
+    const float4 v = reinterpret_cast<const float4*>(v1)[i];
+    float* wf = &w.x; const float* mf = &m.x; const float* vf = &v.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wf[k] = fmaf(step, lamb_dir(mf[k], vf[k], wf[k], h.inv_bc1, h.inv_sqrt_bc2, h.eps, h.wd), wf[k]);
+    reinterpret_cast<float4*>(p)[i] = w;
+    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
+  }
+}
+
 __global__ void cast_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, int64_t n4) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
     store_bf16x4(out, i * 4, reinterpret_cast<const float4*>(x)[i]);
@@ -116,7 +429,56 @@ void sgd_step(float* p, const float* g, float* mom, void* p16, int64_t n, const 
 void adam_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper,
                cudaStream_t s) {
   const int64_t n4 = n / 4;
-  adam_kernel<<<blocks_for(n4), 256, 0, s>>>(p, g, m, v, (__nv_bfloat16*)p16, n4, hyper);
+  adam_kernel<false><<<blocks_for(n4), 256, 0, s>>>(p, g, m, v, (__nv_bfloat16*)p16, n4, hyper);
+}
+void adamw_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper,
+                cudaStream_t s) {
+  const int64_t n4 = n / 4;
+  adam_kernel<true><<<blocks_for(n4), 256, 0, s>>>(p, g, m, v, (__nv_bfloat16*)p16, n4, hyper);
+}
+void rmsprop_step(float* p, const float* g, float* sq, float* mom, float* avg, void* p16, int64_t n,
+                  const float* hyper, cudaStream_t s) {
+  const int64_t n4 = n / 4;
+  auto* b16 = (__nv_bfloat16*)p16;
+  const int nb = blocks_for(n4);
+  if (avg != nullptr && mom != nullptr)
+    rmsprop_kernel<true, true><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
+  else if (avg != nullptr)
+    rmsprop_kernel<true, false><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
+  else if (mom != nullptr)
+    rmsprop_kernel<false, true><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
+  else
+    rmsprop_kernel<false, false><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
+}
+void adagrad_step(float* p, const float* g, float* acc, void* p16, int64_t n, const float* hyper, cudaStream_t s) {
+  const int64_t n4 = n / 4;
+  adagrad_kernel<<<blocks_for(n4), 256, 0, s>>>(p, g, acc, (__nv_bfloat16*)p16, n4, hyper);
+}
+void adamax_step(float* p, const float* g, float* m, float* u, void* p16, int64_t n, const float* hyper,
+                 cudaStream_t s) {
+  const int64_t n4 = n / 4;
+  adamax_kernel<<<blocks_for(n4), 256, 0, s>>>(p, g, m, u, (__nv_bfloat16*)p16, n4, hyper);
+}
+void segment_sumsq(const float* g, int64_t n, const int64_t* chunks, int64_t nchunks, float* partial,
+                   const float* hyper, cudaStream_t s) {
+  segment_sumsq_kernel<<<(unsigned)nchunks, kChunkThreads, 0, s>>>(g, n, chunks, partial, hyper);
+}
+void segment_finalize(const float* partial, int64_t nchunks, const int64_t* segs, int nseg, float* sums,
+                      float* factor, float* hyper, int mode, cudaStream_t s) {
+  segment_finalize_kernel<<<1, kFinThreads, 0, s>>>(partial, nchunks, segs, nseg, sums, factor, hyper, mode);
+}
+void clip_apply(float* g, int64_t n, const int64_t* chunks, int64_t nchunks, const float* factor, int nseg,
+                const float* hyper, cudaStream_t s) {
+  clip_apply_kernel<<<(unsigned)nchunks, kChunkThreads, 0, s>>>(g, n, chunks, factor, nseg, hyper);
+}
+void lamb_moments(const float* p, const float* g, float* m, float* v, int64_t n, const int64_t* chunks,
+                  int64_t nchunks, float* partial, const float* hyper, cudaStream_t s) {
+  lamb_moments_kernel<<<(unsigned)nchunks, kChunkThreads, 0, s>>>(p, g, m, v, n, chunks, nchunks, partial, hyper);
+}
+void lamb_apply(float* p, const float* m, const float* v, void* p16, int64_t n, const int64_t* chunks,
+                int64_t nchunks, const float* phi, int nseg, const float* hyper, cudaStream_t s) {
+  lamb_apply_kernel<<<(unsigned)nchunks, kChunkThreads, 0, s>>>(p, m, v, (__nv_bfloat16*)p16, n, chunks, phi, nseg,
+                                                                hyper);
 }
 void adadelta_step(float* p, const float* g, float* sq, float* acc, void* p16, int64_t n, const float* hyper,
                    cudaStream_t s) {

@@ -907,7 +907,7 @@ class EngineTrainStep:
             e.grad_hook = optimizer.on_grads_ready
         else:
             e.bind_grad_buffer()
-            optimizer.attach(e.params, e.grads, e.w16)
+            optimizer.attach(e.params, e.grads, e.w16, segments=ranges)
         e.build(training=True)
         if self._dist:
             optimizer.extra_wait_streams = list(e.aux_streams)

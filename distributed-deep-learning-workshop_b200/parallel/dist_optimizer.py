@@ -115,8 +115,10 @@ class DistributedOptimizer:
     def allocate_weights(self, params: torch.Tensor, w16: Optional[torch.Tensor]):
         """fused_update only: move the fp32 master (and bf16 copy) into symmetric + multicast memory.  Returns the
         (params, w16) tensors the model must use from now on, or the inputs unchanged when fusion is unavailable."""
+        # the per-bucket kernel sees one bucket at a time, so it cannot apply a clip that needs the whole gradient
         ok = (self.fused_update and self.world > 1 and params.is_cuda and self._sym is not None
-              and self._sym.has_multicast and getattr(self.opt, "name", "") == "SGD" and not self.opt.nesterov)
+              and self._sym.has_multicast and getattr(self.opt, "name", "") == "SGD" and not self.opt.nesterov
+              and getattr(self.opt, "clip_mode", None) is None)
         if not ok:
             self.fused_update = False
             return params, w16
@@ -138,7 +140,7 @@ class DistributedOptimizer:
         if grads is None:
             grads = self.grads if self.grads is not None else self.allocate_grads(params.numel(), params.device)
         self.grads = grads
-        self.opt.attach(params, grads, w16)
+        self.opt.attach(params, grads, w16, segments=spec_ranges)
         self.buckets = []
         elem_budget = max(1, self.bucket_bytes // 4)
         lo = None

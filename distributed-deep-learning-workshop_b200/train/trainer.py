@@ -177,7 +177,7 @@ class _ModuleBackend:
             optimizer.attach(self.flat.params, self.flat.ranges, None, grads)
             self.flat.set_ready_hook(optimizer.on_grads_ready)
         else:
-            optimizer.attach(self.flat.params, self.flat.grads, None)
+            optimizer.attach(self.flat.params, self.flat.grads, None, segments=self.flat.ranges)
         self._results: deque = deque()
         self.batch = None
 
@@ -273,7 +273,12 @@ class Trainer:
     # ------------------------------------------------------------------------------------------------ compile
     def compile(self, optimizer, loss: str = "sparse_categorical_crossentropy", metrics: Sequence[str] = ("accuracy",),
                 **_ignored) -> "Trainer":
-        """`model.compile(optimizer=..., loss=SparseCategoricalCrossentropy(from_logits=True), metrics=['accuracy'])`"""
+        """`model.compile(optimizer=..., loss=SparseCategoricalCrossentropy(from_logits=True), metrics=['accuracy'])`;
+        ``optimizer`` may be a name (``"rmsprop"``, ``"adamw"``, ...): `optim.get(name)()` with Keras's defaults."""
+        if isinstance(optimizer, str):
+            from .. import optim
+
+            optimizer = optim.get(optimizer)()
         loss_name = loss if isinstance(loss, str) else getattr(loss, "name", "sparse_categorical_crossentropy")
         if "sparse_categorical_crossentropy" not in loss_name:
             raise ValueError("only sparse categorical cross-entropy from logits is implemented (what the reference uses)")
