@@ -1,10 +1,9 @@
-// pybind layer for the wgmma convolution kernels: validates tensors, derives the tiling, encodes the TMA
-// descriptors once, and exposes launchable plan objects (static buffers => plans are reused under CUDA graphs).
+// pybind layer for the wgmma convolution kernels: validates tensors and the tiling ops/conv.py planned (rejecting any
+// the kernels cannot run), encodes the TMA descriptors once, and exposes launchable plan objects (static buffers =>
+// plans are reused under CUDA graphs).
 #include <ATen/cuda/CUDAContext.h>
 #include <torch/extension.h>
 
-#include <algorithm>
-#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -47,11 +46,12 @@ struct ConvPlan {
   // views:  1..4 NHWC (possibly strided) input views on one pixel grid (N, Hv, Wv, Cin)
   // weight: bf16 [taps*Cout, Cin];  out: NHWC view (N, Ho, Wo, Cout)
   // tap_map/dw/dh: per tap view index + pixel offset;  bw/bh/bn: pixel box (0 => flat 1x1 mode)
+  // block_n, resident_filter, halo, grid: the rest of the tiling (ops/conv.py plan_conv)
   ConvPlan(std::vector<at::Tensor> views, at::Tensor weight, at::Tensor out, std::vector<int64_t> tap_map,
            std::vector<int64_t> tap_dw, std::vector<int64_t> tap_dh, int64_t bw, int64_t bh, int64_t bn,
-           c10::optional<at::Tensor> stat_sum, c10::optional<at::Tensor> stat_sqsum, int64_t max_ctas,
-           c10::optional<at::Tensor> bwd_y, c10::optional<at::Tensor> bn_scale, c10::optional<at::Tensor> bn_shift,
-           c10::optional<at::Tensor> add_src, c10::optional<at::Tensor> relu_mask, c10::optional<at::Tensor> ep_scale,
+           int64_t block_n, bool resident_filter, bool halo, int64_t grid, c10::optional<at::Tensor> stat_sum,
+           c10::optional<at::Tensor> stat_sqsum, c10::optional<at::Tensor> bwd_y, c10::optional<at::Tensor> bn_scale,
+           c10::optional<at::Tensor> bn_shift, c10::optional<at::Tensor> add_src, c10::optional<at::Tensor> relu_mask, c10::optional<at::Tensor> ep_scale,
            c10::optional<at::Tensor> ep_shift, int64_t ep_act) {
     TORCH_CHECK(!views.empty() && views.size() <= 4, "1..4 input views");
     for (auto& v : views) check_nhwc_view(v, "input view");
@@ -66,9 +66,10 @@ struct ConvPlan {
     TORCH_CHECK(weight.is_cuda() && weight.scalar_type() == at::kBFloat16 && weight.is_contiguous() &&
                     weight.dim() == 2 && weight.size(0) == taps * cout && weight.size(1) == cin,
                 "weight must be bf16 [taps*Cout, Cin]");
+    TORCH_CHECK((block_n == 64 || block_n == 128) && cout % block_n == 0, "block_n must be 64 or 128 and divide Cout");
     ConvParams& p = raw.p;
     std::memset(&p, 0, sizeof(p));
-    raw.block_n = cout % 128 == 0 ? 128 : 64;
+    raw.block_n = (int)block_n;
     p.taps = taps;
     p.kblocks = (int)(cin / 64);
     p.cout = (int)cout;
@@ -111,63 +112,39 @@ struct ConvPlan {
       }
       raw.tmD = map_nhwc(out, 64, (int)bw, (int)bh, (int)bn);
     }
-    // Tile width: the wider N tile re-reads the A operand less, but a persistent grid of one CTA per SM pays for whole
-    // waves.  The cost model is waves x tile width (the MMA time of a tile is proportional to its width); the narrower
-    // tile is taken only when it wins by >= 10 %.  128 is the widest: each consumer warpgroup holds a whole tile's
-    // 128 x BLOCK_N fp32 accumulator in registers (128 per thread at BLOCK_N = 128).  B200DDL_BLOCK_N=128|64 forces a
-    // width (A/B measurements).
-    {
-      const int cap_ = max_ctas > 0 ? (int)max_ctas : sm_count();
-      auto cost = [&](int bn) {
-        const int64_t tiles = (int64_t)p.m_tiles * (cout / bn);
-        return ((tiles + cap_ - 1) / cap_) * bn;
-      };
-      int best = raw.block_n;
-      for (int bn = raw.block_n / 2; bn >= 64; bn /= 2)
-        if (cout % bn == 0 && cost(bn) * 10 <= cost(best) * 9) best = bn;
-      if (const char* f = std::getenv("B200DDL_BLOCK_N")) {
-        const int v = std::atoi(f);
-        if ((v == 128 || v == 64) && cout % v == 0) best = v;
-      }
-      raw.block_n = best;
-    }
     p.n_blocks = (int)(cout / raw.block_n);
     raw.tmB = map_2d(weight.data_ptr(), taps * cout, cin, cin, 64, raw.block_n);
     p.num_tiles = p.m_tiles * p.n_blocks;
     raw.stats = stat_sum.has_value() ? (bwd_y.has_value() ? (relu_mask.has_value() ? 3 : 2) : 1) : (ep_scale.has_value() ? 4 : 0);
     p.m_rows = N * Ho * Wo;
     // Resident filter: one N-block of 64 channels whose taps * kblocks filter tiles (8 KB each) fit in 72 KB.
-    // B200DDL_NO_RESIDENT_FILTER=1 switches it off (A/B measurements).
-    {
-      const char* off = std::getenv("B200DDL_NO_RESIDENT_FILTER");
-      raw.res_b = (raw.block_n == 64 && p.n_blocks == 1 && taps * p.kblocks <= 9 && !(off && off[0] == '1') &&
-                   raw.stats != 3) ? 1 : 0;
-    }
+    TORCH_CHECK(!resident_filter || (raw.block_n == 64 && p.n_blocks == 1 && taps * p.kblocks <= 9 && raw.stats != 3),
+                "a resident filter needs one 64-channel N-block of <= 9 filter tiles and no block-gradient epilogue");
+    raw.res_b = resident_filter ? 1 : 0;
     // Halo mode: a 3x3 stride-1 conv (9 taps on ONE view forming the full {-1,0,1}^2 offset grid, in any order) over
     // full-width single-image boxes: one [bw x (bh+2)] load per horizontal offset serves its three vertical taps, read at
     // row offsets 0 / bw / 2*bw - whole 1024 B swizzle atoms only when bw % 8 == 0.
-    // B200DDL_NO_HALO=1 switches it off (A/B measurements).
-    raw.halo = 0;
-    {
-      const char* off = std::getenv("B200DDL_NO_HALO");
-      bool ok = raw.res_b && p.mode == 1 && taps == 9 && views.size() == 1 && bn == 1 && !(off && off[0] == '1') &&
-                bw % 8 == 0 && bw == views[0].size(2) && bw == Wo && bw * (bh + 2) <= 224;
+    raw.halo = halo ? 1 : 0;
+    if (halo) {
+      TORCH_CHECK(resident_filter && p.mode == 1 && taps == 9 && views.size() == 1,
+                  "halo mode needs a resident filter and 9 taps on one view in box mode");
+      TORCH_CHECK(bw == views[0].size(2) && bw == Wo && bw % 8 == 0 && bn == 1 && bw * (bh + 2) <= 224,
+                  "halo mode needs a full-width single-image box, width % 8 == 0, of <= 224 pixels with its halo rows");
       int8_t table[9];
       for (int i = 0; i < 9; ++i) table[i] = -1;
-      for (int t = 0; ok && t < 9; ++t) {
+      for (int t = 0; t < 9; ++t) {
         const int dwv = p.tap_dw[t], dhv = p.tap_dh[t];
-        if (p.tap_map[t] != 0 || dwv < -1 || dwv > 1 || dhv < -1 || dhv > 1 || table[(dwv + 1) * 3 + (dhv + 1)] != -1) ok = false;
-        else table[(dwv + 1) * 3 + (dhv + 1)] = (int8_t)t;
+        TORCH_CHECK(p.tap_map[t] == 0 && dwv >= -1 && dwv <= 1 && dhv >= -1 && dhv <= 1 &&
+                        table[(dwv + 1) * 3 + (dhv + 1)] == -1,
+                    "halo mode needs the taps to form the 3x3 offset grid");
+        table[(dwv + 1) * 3 + (dhv + 1)] = (int8_t)t;
       }
-      if (ok) {
-        raw.halo = 1;
-        p.halo = 1;
-        p.halo_bytes = (int)(bw * (bh + 2) * 128);
-        p.halo_dh0 = -1;
-        for (int hs = 0; hs < 3; ++hs) p.halo_dw[hs] = (int8_t)(hs - 1);
-        for (int i = 0; i < 9; ++i) p.halo_tap[i] = table[i];
-        raw.tmA[1] = map_nhwc(views[0], 64, (int)bw, (int)bh + 2, 1);
-      }
+      p.halo = 1;
+      p.halo_bytes = (int)(bw * (bh + 2) * 128);
+      p.halo_dh0 = -1;
+      for (int hs = 0; hs < 3; ++hs) p.halo_dw[hs] = (int8_t)(hs - 1);
+      for (int i = 0; i < 9; ++i) p.halo_tap[i] = table[i];
+      raw.tmA[1] = map_nhwc(views[0], 64, (int)bw, (int)bh + 2, 1);
     }
     raw.tmY = raw.tmD;
     if (raw.stats == 3) {
@@ -242,8 +219,8 @@ struct ConvPlan {
       keep.push_back(*stat_sum);
       keep.push_back(*stat_sqsum);
     }
-    const int cap = max_ctas > 0 ? (int)max_ctas : sm_count();
-    raw.grid = p.num_tiles < cap ? p.num_tiles : cap;
+    TORCH_CHECK(grid >= 1 && grid <= p.num_tiles, "grid must be 1..tiles CTAs");
+    raw.grid = (int)grid;
     for (auto& v : views) keep.push_back(v);
     keep.push_back(weight);
     keep.push_back(out);
@@ -325,7 +302,7 @@ struct WgradPlan {
   // dy: NHWC view (N, Ho, Wo, Cout) bf16;  views: input views on the same pixel grid;  dw: fp32 [taps*Cout, Cin]
   WgradPlan(at::Tensor dy, std::vector<at::Tensor> views, at::Tensor dw, int64_t R, int64_t S,
             std::vector<int64_t> tap_map, std::vector<int64_t> tap_dw, std::vector<int64_t> tap_dh, int64_t bw,
-            int64_t bh, int64_t bn, int64_t px_chunks, int64_t max_ctas, int64_t smem_budget) {
+            int64_t bh, int64_t bn, int64_t cb_per_group, int64_t stages, int64_t px_chunks, int64_t grid) {
     check_nhwc_view(dy, "dy");
     TORCH_CHECK(!views.empty() && views.size() <= 4);
     for (auto& v : views) check_nhwc_view(v, "input view");
@@ -337,7 +314,6 @@ struct WgradPlan {
     TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.is_contiguous() && dw.numel() == taps * cout * cin,
                 "dw must be fp32 [taps*Cout, Cin]");
     TORCH_CHECK(S >= 1 && S <= 4, "filter width 1..4");
-    // the unit's 64 x (64 * G) fp32 accumulator lives in the registers of one warpgroup: G <= 4 (N <= 256)
     WgradParams& p = raw.p;
     std::memset(&p, 0, sizeof(p));
     p.cout = (int)cout;
@@ -346,12 +322,10 @@ struct WgradPlan {
     p.a_chunks = cout == 64 ? 1 : 2;
     p.co_blocks = (int)((cout + 127) / 128);
     const int cin_blocks = (int)(cin / 64);
-    if (S == 1) {
-      p.cb_per_group = cin_blocks < 4 ? cin_blocks : 4;
-      while (cin_blocks % p.cb_per_group) --p.cb_per_group;
-    } else {
-      p.cb_per_group = (cin_blocks >= 2 && S * 2 <= 4) ? 2 : 1;
-    }
+    // the unit's 64 x (64 * G) fp32 accumulator lives in the registers of one warpgroup: G <= 4 (N <= 256)
+    TORCH_CHECK(cb_per_group >= 1 && cin_blocks % cb_per_group == 0 && S * cb_per_group <= 4,
+                "cb_per_group must divide Cin / 64 with S * cb_per_group <= 4");
+    p.cb_per_group = (int)cb_per_group;
     p.G = (int)S * p.cb_per_group;
     p.cgroups = cin_blocks / p.cb_per_group;
     p.groups = (int)R * p.cgroups;
@@ -391,23 +365,18 @@ struct WgradPlan {
         raw.tmX[i] = map_nhwc(v, 64, (int)bw, (int)bh, (int)bn);
       }
     }
-    const int stage_bytes = (p.a_chunks + p.G) * p.P * 128;
-    // smem_budget < 227 KB leaves room for bandwidth-bound kernels to co-reside when wgrad runs on a side stream
-    const int budget = (smem_budget > 0 && smem_budget < 232448) ? (int)smem_budget : 232448;
-    p.stages = (budget - 256 - 1024) / stage_bytes;   // + barriers, + 1 KB to align the dynamic smem base
-    if (p.stages > 8) p.stages = 8;
-    TORCH_CHECK(p.stages >= 2, "wgrad stage does not fit shared memory");
-    const int combos = p.co_blocks * p.groups;
-    const int cap = max_ctas > 0 ? (int)max_ctas : sm_count();
-    // one wave of units: every extra pixel chunk costs a full accumulator flush of fp32 atomics
-    int64_t pc = px_chunks > 0 ? px_chunks : cap / combos;
-    if (pc < 1) pc = 1;
-    if (pc > p.iters_total) pc = p.iters_total;
-    p.iters_per_chunk = (int)((p.iters_total + pc - 1) / pc);
+    // + barriers, + 1 KB to align the dynamic smem base
+    const int64_t smem = stages * (p.a_chunks + p.G) * p.P * 128 + 256 + 1024;
+    TORCH_CHECK(stages >= 2 && stages <= 8 && smem <= 232448, "wgrad needs 2..8 stages in 227 KB of shared memory");
+    p.stages = (int)stages;
+    TORCH_CHECK(px_chunks >= 1 && px_chunks <= p.iters_total, "px_chunks must be 1..pixel iterations");
+    p.iters_per_chunk = (int)((p.iters_total + px_chunks - 1) / px_chunks);
     p.px_chunks = (p.iters_total + p.iters_per_chunk - 1) / p.iters_per_chunk;
-    p.num_units = p.px_chunks * combos;
+    TORCH_CHECK(p.px_chunks == px_chunks, "px_chunks leaves a pixel chunk empty");
+    p.num_units = p.px_chunks * p.co_blocks * p.groups;
     p.dw = dw.data_ptr<float>();
-    raw.grid = p.num_units < cap ? p.num_units : cap;
+    TORCH_CHECK(grid >= 1 && grid <= p.num_units, "grid must be 1..units CTAs");
+    raw.grid = (int)grid;
     keep.push_back(dy);
     for (auto& v : views) keep.push_back(v);
     keep.push_back(dw);
@@ -492,13 +461,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "b200ddl wgmma/TMA implicit-GEMM convolution kernels (sm_90a)";
   py::class_<b200::ConvPlan>(m, "ConvPlan")
       .def(py::init<std::vector<at::Tensor>, at::Tensor, at::Tensor, std::vector<int64_t>, std::vector<int64_t>,
-                    std::vector<int64_t>, int64_t, int64_t, int64_t, c10::optional<at::Tensor>,
-                    c10::optional<at::Tensor>, int64_t, c10::optional<at::Tensor>, c10::optional<at::Tensor>,
+                    std::vector<int64_t>, int64_t, int64_t, int64_t, int64_t, bool, bool, int64_t,
+                    c10::optional<at::Tensor>, c10::optional<at::Tensor>, c10::optional<at::Tensor>,
                     c10::optional<at::Tensor>, c10::optional<at::Tensor>, c10::optional<at::Tensor>, c10::optional<at::Tensor>,
-                    c10::optional<at::Tensor>, int64_t>(),
+                    c10::optional<at::Tensor>, c10::optional<at::Tensor>, int64_t>(),
            py::arg("views"), py::arg("weight"), py::arg("out"), py::arg("tap_map"), py::arg("tap_dw"),
-           py::arg("tap_dh"), py::arg("bw"), py::arg("bh"), py::arg("bn"), py::arg("stat_sum") = c10::nullopt,
-           py::arg("stat_sqsum") = c10::nullopt, py::arg("max_ctas") = 0, py::arg("bwd_y") = c10::nullopt,
+           py::arg("tap_dh"), py::arg("bw"), py::arg("bh"), py::arg("bn"), py::arg("block_n"),
+           py::arg("resident_filter"), py::arg("halo"), py::arg("grid"), py::arg("stat_sum") = c10::nullopt,
+           py::arg("stat_sqsum") = c10::nullopt, py::arg("bwd_y") = c10::nullopt,
            py::arg("bn_scale") = c10::nullopt, py::arg("bn_shift") = c10::nullopt, py::arg("add_src") = c10::nullopt,
            py::arg("relu_mask") = c10::nullopt, py::arg("ep_scale") = c10::nullopt, py::arg("ep_shift") = c10::nullopt,
            py::arg("ep_act") = 0)
@@ -516,10 +486,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
       .def_property_readonly("stats_mode", &b200::ConvPlan::stats_mode);
   py::class_<b200::WgradPlan>(m, "WgradPlan")
       .def(py::init<at::Tensor, std::vector<at::Tensor>, at::Tensor, int64_t, int64_t, std::vector<int64_t>,
-                    std::vector<int64_t>, std::vector<int64_t>, int64_t, int64_t, int64_t, int64_t, int64_t, int64_t>(),
+                    std::vector<int64_t>, std::vector<int64_t>, int64_t, int64_t, int64_t, int64_t, int64_t, int64_t,
+                    int64_t>(),
            py::arg("dy"), py::arg("views"), py::arg("dw"), py::arg("R"), py::arg("S"), py::arg("tap_map"),
-           py::arg("tap_dw"), py::arg("tap_dh"), py::arg("bw"), py::arg("bh"), py::arg("bn"),
-           py::arg("px_chunks") = 0, py::arg("max_ctas") = 0, py::arg("smem_budget") = 0)
+           py::arg("tap_dw"), py::arg("tap_dh"), py::arg("bw"), py::arg("bh"), py::arg("bn"), py::arg("cb_per_group"),
+           py::arg("stages"), py::arg("px_chunks"), py::arg("grid"))
       .def("run", &b200::WgradPlan::run)
       .def_readonly("launches", &b200::WgradPlan::launches)
       .def_property_readonly("grid", &b200::WgradPlan::grid)

@@ -29,7 +29,7 @@ struct ConvParams {
   const float* bn_shift;
   // Halo mode (3x3 stride 1, full-width pixel boxes, resident filter): ONE [bw x (bh+2)] box per horizontal tap offset
   // (tensor map 1 of the A array) serves the three vertical taps at row offsets 0, bw, 2*bw of the stage.
-  int halo;              // 0 off, 1 vertical halo (3 loads per tile), 2 two-dimensional halo (1 load per tile, bw == 8)
+  int halo;              // 0 off, 1 on (3 loads per tile)
   int halo_bytes;        // bw * (bh + 2) * 128
   int8_t halo_dw[3];     // horizontal offset of stage s
   int8_t halo_dh0;       // vertical offset of row-shift 0 (normally -1)

@@ -58,22 +58,137 @@ def pick_box(n: int, h: int, w: int, rows: int = 128, multiple_of: int = 1) -> T
     return best[1]
 
 
-def halo_box(h: int, w: int, cin: int, cout: int, R: int, S: int, stride: int, pad: int) -> Optional[Tuple[int, int, int]]:
-    """Full-width single-image box (w, bh, 1) for the kernel's halo mode, or None when the layer does not qualify.
+def halo_box(h: int, w: int) -> Optional[Tuple[int, int, int]]:
+    """Full-width single-image box (w, bh, 1) for the kernel's halo mode, or None when the output plane has none.
 
-    Halo mode (csrc/conv_igemm.cuh): 3x3 / stride 1 / pad 1 with a resident 64x64 filter; one [w x (bh+2)] load per
-    horizontal tap offset serves the three vertical taps, so a stage (28 KB) must hold w * (bh + 2) <= 224 pixels and the
-    MMA tile w * bh <= 128; the vertical taps start w and 2*w rows into the stage, which must be whole 8-row swizzle atoms
-    (w % 8 == 0).  `B200DDL_NO_HALO=1` keeps the generic boxes (A/B measurements)."""
-    if os.environ.get("B200DDL_NO_HALO") == "1" or os.environ.get("B200DDL_NO_RESIDENT_FILTER") == "1":
+    Halo mode (csrc/conv_igemm.cuh): one [w x (bh+2)] load per horizontal tap offset serves the three vertical taps, so a
+    stage (28 KB) must hold w * (bh + 2) <= 224 pixels and the MMA tile w * bh <= 128; the vertical taps start w and 2*w
+    rows into the stage, which must be whole 8-row swizzle atoms (w % 8 == 0)."""
+    if w % 8:
         return None
-    if not (R == 3 and S == 3 and stride == 1 and pad == 1 and cin == 64 and cout == 64 and w % 8 == 0):
-        return None
-    best = None
-    for bh in _divisors(h):
-        if w * bh <= 128 and w * (bh + 2) <= 224:
-            best = bh if best is None else max(best, bh)
-    return None if best is None else (w, best, 1)
+    bhs = [bh for bh in _divisors(h) if w * bh <= 128 and w * (bh + 2) <= 224]
+    return (w, max(bhs), 1) if bhs else None
+
+
+@dataclass(frozen=True)
+class ConvSwitches:
+    """A/B switches of the convolution planner, for measurements; the defaults give the production plans."""
+    block_n: int = 0                  # 64 or 128: force this N-tile width wherever it divides Cout
+    no_halo: bool = False             # no halo mode
+    no_resident_filter: bool = False  # no resident filter (and so no halo mode)
+
+
+def conv_switches() -> ConvSwitches:
+    """The switches from the environment: ``B200DDL_BLOCK_N=64|128``, ``B200DDL_NO_HALO=1``,
+    ``B200DDL_NO_RESIDENT_FILTER=1``."""
+    block_n = os.environ.get("B200DDL_BLOCK_N", "")
+    return ConvSwitches(block_n=int(block_n) if block_n in ("64", "128") else 0,
+                        no_halo=os.environ.get("B200DDL_NO_HALO") == "1",
+                        no_resident_filter=os.environ.get("B200DDL_NO_RESIDENT_FILTER") == "1")
+
+
+def sm_count() -> int:
+    """SMs of the current device: the persistent grid of a plan without ``max_ctas`` has one CTA per SM."""
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
+@dataclass(frozen=True)
+class ConvTiling:
+    box: Tuple[int, int, int]   # pixel box (bw, bh, bn); (0, 0, 0) = flat
+    block_n: int                # N-tile width (output channels per tile)
+    resident_filter: bool       # the CTA's whole filter slice stays in shared memory
+    halo: bool                  # halo mode (3x3 stride-1 taps over full-width boxes)
+    tiles: int                  # M-tiles x N-blocks
+    grid: int                   # persistent CTAs
+
+
+_HALO_OFFSETS = sorted((dw, dh) for dw in (-1, 0, 1) for dh in (-1, 0, 1))
+
+
+def plan_conv(grid: Sequence[int], view_widths: Sequence[int], cin: int, cout: int, tap_map: Sequence[int],
+              tap_dw: Sequence[int], tap_dh: Sequence[int], flat: bool, stats_mode: int, max_ctas: int, sm_count: int,
+              switches: ConvSwitches) -> ConvTiling:
+    """Tiling of one implicit-GEMM convolution (csrc/conv_igemm.cuh) writing an (N, Ho, Wo, cout) ``grid`` from input
+    views of widths ``view_widths`` through the given tap table; ``flat``: a dense 1x1 GEMM over all pixels.
+    ``stats_mode`` is the epilogue (0 none, 1 forward statistics, 2 fused BatchNorm-backward reduction, 3 block-gradient
+    merge, 4 inference epilogue); ``max_ctas`` (0: ``sm_count``) caps the persistent grid."""
+    n, ho, wo = grid
+    taps = len(tap_map)
+    cap = max_ctas if max_ctas > 0 else sm_count
+    # Resident filter: one N-block of 64 channels whose taps * kblocks filter tiles (8 KB each) fit in 72 KB.
+    resident = cout == 64 and taps * (cin // 64) <= 9 and stats_mode != 3 and not switches.no_resident_filter
+    # Halo mode: 9 taps on ONE view of the output's width forming the full {-1,0,1}^2 offset grid, in any order.
+    halo = (resident and not switches.no_halo and not flat and len(view_widths) == 1 and view_widths[0] == wo
+            and not any(tap_map) and sorted(zip(tap_dw, tap_dh)) == _HALO_OFFSETS)
+    box = halo_box(ho, wo) if halo else None
+    halo = box is not None
+    if flat:
+        box = (0, 0, 0)
+        m_tiles = -(-n * ho * wo // 128)
+    else:
+        box = box or pick_box(n, ho, wo)
+        m_tiles = (wo // box[0]) * (ho // box[1]) * -(-n // box[2])
+    # Tile width: the wider N tile re-reads the A operand less, but a persistent grid of one CTA per SM pays for whole
+    # waves.  The cost model is waves x tile width (the MMA time of a tile is proportional to its width); the narrower
+    # tile is taken only when it wins by >= 10 %.  128 is the widest: each consumer warpgroup holds a whole tile's
+    # 128 x BLOCK_N fp32 accumulator in registers (128 per thread at BLOCK_N = 128).
+    def cost(bn: int) -> int:
+        return -(-m_tiles * (cout // bn) // cap) * bn
+
+    block_n = 128 if cout % 128 == 0 and cost(64) * 10 > cost(128) * 9 else 64
+    if switches.block_n and cout % switches.block_n == 0:
+        block_n = switches.block_n
+    tiles = m_tiles * (cout // block_n)
+    return ConvTiling(box, block_n, resident, halo, tiles, min(tiles, cap))
+
+
+SMEM_BYTES = 232448   # 227 KB: the largest dynamic shared memory of one CTA on sm_90
+_WG_SMEM_EXTRA = 256 + 1024   # mbarriers, and 1 KB to align the dynamic smem base
+
+
+@dataclass(frozen=True)
+class WgradTiling:
+    box: Tuple[int, int, int]   # pixel box (bw, bh, bn) of one k-iteration; (0, 0, 0) = flat (64 pixels)
+    cb_per_group: int           # Cin 64-blocks per unit
+    G: int                      # 64-channel X chunks per unit: S * cb_per_group
+    stages: int                 # pipeline stages
+    px_chunks: int              # split-K factor over pixels
+    units: int
+    grid: int                   # persistent CTAs
+
+
+def plan_wgrad(grid: Sequence[int], cin: int, cout: int, R: int, S: int, flat: bool, px_chunks: int, max_ctas: int,
+               smem_budget: int, sm_count: int) -> WgradTiling:
+    """Tiling of one weight-gradient GEMM (csrc/conv_wgrad.cu) over the (N, Ho, Wo) ``grid`` of dy: a unit is one filter
+    row, one Cin group and one 128-channel Cout block over one pixel chunk.  ``px_chunks`` (0: one wave of units),
+    ``max_ctas`` (0: ``sm_count``) and ``smem_budget`` (0: all of it) are the caller's limits."""
+    n, ho, wo = grid
+    cb = cin // 64
+    # the unit's 64 x (64 * G) fp32 accumulator lives in the registers of one warpgroup: G <= 4 (N <= 256)
+    cb_per_group = max(d for d in (1, 2, 3, 4) if cb % d == 0) if S == 1 else (2 if cb >= 2 and S * 2 <= 4 else 1)
+    G = S * cb_per_group
+    chunks = (1 if cout == 64 else 2) + G   # 64-channel chunks of a stage: dY's, then X's
+    # smem_budget < 227 KB leaves room for bandwidth-bound kernels to co-reside when wgrad runs on a side stream
+    budget = smem_budget if 0 < smem_budget < SMEM_BYTES else SMEM_BYTES
+    if flat:
+        box, P = (0, 0, 0), 64
+        iters = n * ho * wo // P
+    else:
+        # keep >= 3 pipeline stages (2 in a budget below 200,000 B): a stage is chunks * P pixels * 128 B
+        want_stages = 3 if budget >= 200000 else 2
+        rows = min(128, ((budget - _WG_SMEM_EXTRA) // (want_stages * chunks * 128)) // 16 * 16)
+        box = pick_box(n, ho, wo, rows=rows, multiple_of=16)
+        P = box[0] * box[1] * box[2]
+        iters = (wo // box[0]) * (ho // box[1]) * -(-n // box[2])
+    stages = min(8, (budget - _WG_SMEM_EXTRA) // (chunks * P * 128))
+    combos = -(-cout // 128) * R * (cb // cb_per_group)
+    cap = max_ctas if max_ctas > 0 else sm_count
+    # one wave of units: every extra pixel chunk costs a full accumulator flush of fp32 atomics
+    pc = min(max(px_chunks if px_chunks > 0 else cap // combos, 1), iters)
+    per_chunk = -(-iters // pc)
+    pc = -(-iters // per_chunk)
+    units = pc * combos
+    return WgradTiling(box, cb_per_group, G, stages, pc, units, min(units, cap))
 
 
 @dataclass
@@ -116,6 +231,22 @@ def make_taps(x: torch.Tensor, R: int, S: int, stride: int, pad: int) -> TapTabl
     return TapTable(views, tm, dw, dh)
 
 
+def _conv_plan(views: List[torch.Tensor], weight: torch.Tensor, out: torch.Tensor, tap_map: List[int],
+               tap_dw: List[int], tap_dh: List[int], flat: bool, stats_mode: int, max_ctas: int, **epilogue):
+    """Plans one implicit GEMM writing ``out`` and builds its launchable binding: (pixel box, plan).  ``epilogue``: the
+    tensors of ``stats_mode``, as the binding names them."""
+    N, Ho, Wo, cout = out.shape
+    t = plan_conv(grid=(N, Ho, Wo), view_widths=[v.shape[2] for v in views], cin=views[0].shape[3], cout=cout,
+                  tap_map=tap_map, tap_dw=tap_dw, tap_dh=tap_dh, flat=flat, stats_mode=stats_mode, max_ctas=max_ctas,
+                  sm_count=sm_count(), switches=conv_switches())
+    bw, bh, bn = t.box
+    plan = _build.load("_b200_conv").ConvPlan(
+        views, weight, out, tap_map, tap_dw, tap_dh, bw=bw, bh=bh, bn=bn, block_n=t.block_n,
+        resident_filter=t.resident_filter, halo=t.halo, grid=t.grid, **epilogue)
+    _plans.add(plan)
+    return t.box, plan
+
+
 class ConvForward:
     """y = conv(x, w) [+ per-channel sum / sum-of-squares of y for BatchNorm] on the tensor cores.
 
@@ -127,29 +258,22 @@ class ConvForward:
         """``epilogue=(scale, shift, act, residual)`` (inference): y = act(conv(x, w) * scale[c] + shift[c] [+ residual])
         with act in {'none', 'relu', 'relu6'} computed in the GEMM epilogue (folded BatchNorm); the residual (a tensor of
         y's shape) needs a dense 1x1 stride-1 convolution.  Mutually exclusive with the statistics outputs."""
-        ext = _build.load("_b200_conv")
         taps = make_taps(x, R, S, stride, pad)
-        N, Ho, Wo, _ = y.shape
         flat = (R == 1 and S == 1 and stride == 1 and pad == 0 and x.is_contiguous() and y.is_contiguous())
-        if flat:
-            bw = bh = bn = 0
-        else:
-            cout_, cin_ = w.shape[0] // (R * S), w.shape[1]
-            bw, bh, bn = halo_box(Ho, Wo, cin_, cout_, R, S, stride, pad) or pick_box(N, Ho, Wo)
-        self.box = (bw, bh, bn)
         if epilogue is not None:
             if stat_sum is not None:
                 raise ValueError("epilogue and statistics outputs are mutually exclusive")
             scale, shift, act, residual = epilogue
             if residual is not None and not flat:
                 raise ValueError("an epilogue residual needs a dense 1x1 stride-1 convolution")
-            self.plan = ext.ConvPlan(taps.views, w, y, taps.tap_map, taps.tap_dw, taps.tap_dh, bw, bh, bn, None, None,
-                                     max_ctas, None, None, None, residual, None, scale, shift,
-                                     {"none": 0, "relu": 1, "relu6": 2}[act])
+            stats_mode = 4
+            outputs = dict(add_src=residual, ep_scale=scale, ep_shift=shift,
+                           ep_act={"none": 0, "relu": 1, "relu6": 2}[act])
         else:
-            self.plan = ext.ConvPlan(taps.views, w, y, taps.tap_map, taps.tap_dw, taps.tap_dh, bw, bh, bn,
-                                     stat_sum, stat_sqsum, max_ctas)
-        _plans.add(self.plan)
+            stats_mode = 0 if stat_sum is None else 1
+            outputs = dict(stat_sum=stat_sum, stat_sqsum=stat_sqsum)
+        self.box, self.plan = _conv_plan(taps.views, w, y, taps.tap_map, taps.tap_dw, taps.tap_dh, flat, stats_mode,
+                                         max_ctas, **outputs)
 
     def run(self) -> None:
         self.plan.run()
@@ -162,18 +286,29 @@ class ConvDgrad:
     needs are (re)built by :meth:`refresh_weights` (cheap: filters are tiny next to activations)."""
 
     @staticmethod
-    def part_taps(R: int, S: int, stride: int, pad: int) -> List[List[int]]:
-        """Filter-tap index lists of the GEMMs a dgrad is made of, in plan order: one list with every tap for stride 1,
-        one list per non-empty output-parity class for stride 2.  (Lets an owner lay all weight copies out in one buffer.)"""
-        if stride == 1:
-            return [[r * S + s for r in range(R) for s in range(S)]]
+    def parity_parts(R: int, S: int, stride: int, pad: int):
+        """The output-parity classes a dgrad is made of, in plan order: ((ph, pw), filter-tap indices, tap offsets dw,
+        dh) with dx[stride*i + ph, stride*j + pw] = sum over the class's taps of dy[i + dh, j + dw] w[tap].  Stride 1 is
+        one class of every tap (the forward conv with the taps reversed); a stride-2 class may have no taps."""
         parts = []
-        for ph in range(2):
-            for pw in range(2):
-                idx = [r * S + s for r in range(R) for s in range(S) if (r - pad) % 2 == ph and (s - pad) % 2 == pw]
-                if idx:
-                    parts.append(idx)
+        for ph in range(stride):
+            for pw in range(stride):
+                idx, dw, dh = [], [], []
+                for r in range(R):
+                    for s in range(S):
+                        oh, ow = r - pad, s - pad
+                        if oh % stride == ph and ow % stride == pw:
+                            idx.append(r * S + s)
+                            dh.append(-((oh - ph) // stride))
+                            dw.append(-((ow - pw) // stride))
+                parts.append(((ph, pw), idx, dw, dh))
         return parts
+
+    @staticmethod
+    def part_taps(R: int, S: int, stride: int, pad: int) -> List[List[int]]:
+        """Filter-tap index lists of the GEMMs a dgrad is made of, in plan order: one list per non-empty output-parity
+        class.  (Lets an owner lay all weight copies out in one buffer.)"""
+        return [idx for _, idx, _, _ in ConvDgrad.parity_parts(R, S, stride, pad) if idx]
 
     def __init__(self, dy: torch.Tensor, w_master: torch.Tensor, dx: torch.Tensor, R: int, S: int, stride: int = 1,
                  pad: int = 0, max_ctas: int = 0, wbuf: Optional[torch.Tensor] = None, bwd_stats=None,
@@ -189,15 +324,12 @@ class ConvDgrad:
             raise ValueError("bwd_stats: stride-1 convs only (a strided dgrad has no fused reduction)")
         if block_grad is not None and (stride != 1 or bwd_stats is not None):
             raise ValueError("block_grad: stride-1 convs only, and not together with bwd_stats")
-        ext = _build.load("_b200_conv")
         self.R, self.S, self.stride, self.pad = R, S, stride, pad
         self.fused_bwd_stats = bwd_stats is not None
         self.block_grad = block_grad is not None
         self.w_master = w_master
         if wbufs is not None:
             assert wbuf is None and len(wbufs) == len(self.part_taps(R, S, stride, pad))
-            if stride == 1:
-                wbuf = wbufs[0]
         self.external_wbuf = wbuf is not None or wbufs is not None  # owner refreshes them (one batched kernel for all layers)
         taps_total, cout, cin = w_master.shape
         assert taps_total == R * S
@@ -206,64 +338,33 @@ class ConvDgrad:
         self._idx_dev = {}
         self.needs_zero = False
         self.dx = dx
-        N, Ho, Wo, _ = dy.shape
-        if stride == 1:
-            # dx[h] = sum_r dy[h + pad - r] w[r]  -> forward conv with taps reversed and pad' = R-1-pad
-            idx = [r * S + s for r in range(R) for s in range(S)]
-            tm, dw, dh = [], [], []
-            for r in range(R):
-                for s in range(S):
-                    tm.append(0)
-                    dh.append(pad - r)
-                    dw.append(pad - s)
-            if wbuf is None:
-                wbuf = torch.empty(len(idx) * cin, cout, dtype=torch.bfloat16, device=dy.device)
+        flat = (R == 1 and S == 1 and stride == 1 and pad == 0 and dy.is_contiguous() and dx.is_contiguous())
+        stats_mode, outputs = 0, {}
+        if block_grad is not None:
+            if not flat:
+                raise ValueError("block_grad needs a dense 1x1 stride-1 convolution")
+            skip, mask, y3, s_dz, s_dzy = block_grad
+            stats_mode, outputs = 3, dict(stat_sum=s_dz, stat_sqsum=s_dzy, bwd_y=y3, add_src=skip, relu_mask=mask)
+        elif bwd_stats is not None:
+            y, sc, sh, s_dz, s_dzy = bwd_stats
+            stats_mode, outputs = 2, dict(stat_sum=s_dz, stat_sqsum=s_dzy, bwd_y=y, bn_scale=sc, bn_shift=sh)
+        for (ph, pw), idx, dw, dh in self.parity_parts(R, S, stride, pad):
+            if not idx:
+                self.needs_zero = True
+                continue
+            if wbufs is not None:
+                buf = wbufs[len(self.parts)]
+            elif wbuf is not None and stride == 1:
+                buf = wbuf
             else:
-                wbuf = wbuf.view(len(idx) * cin, cout)
-            flat = (R == 1 and S == 1 and pad == 0 and dy.is_contiguous() and dx.is_contiguous())
-            box = (0, 0, 0) if flat else (halo_box(dx.shape[1], dx.shape[2], cout, cin, R, S, 1, R - 1 - pad)
-                                          or pick_box(N, dx.shape[1], dx.shape[2]))
-            if block_grad is not None:
-                if not flat:
-                    raise ValueError("block_grad needs a dense 1x1 stride-1 convolution")
-                skip, mask, y3, s_dz, s_dzy = block_grad
-                plan = ext.ConvPlan([dy], wbuf, dx, tm, dw, dh, 0, 0, 0, s_dz, s_dzy, max_ctas, y3, None, None,
-                                    skip, mask)
-            elif self.fused_bwd_stats:
-                y, sc, sh, s_dz, s_dzy = bwd_stats
-                plan = ext.ConvPlan([dy], wbuf, dx, tm, dw, dh, box[0], box[1], box[2], s_dz, s_dzy, max_ctas, y, sc, sh)
-            else:
-                plan = ext.ConvPlan([dy], wbuf, dx, tm, dw, dh, box[0], box[1], box[2], None, None, max_ctas)
-            _plans.add(plan)
-            self.parts.append((plan, wbuf, idx))
+                buf = torch.empty(len(idx) * cin, cout, dtype=torch.bfloat16, device=dy.device)
+                if stride != 1:
+                    self._idx_dev[tuple(idx)] = torch.tensor(idx, device=dy.device, dtype=torch.long)
+            buf = buf.view(len(idx) * cin, cout)
+            box, plan = _conv_plan([dy], buf, dx[:, ph::stride, pw::stride, :], [0] * len(idx), dw, dh, flat,
+                                   stats_mode, max_ctas, **outputs)
+            self.parts.append((plan, buf, idx))
             self.boxes.append(box)
-        else:
-            # output parity classes: dx[2i+ph, 2j+pw] = sum_{taps with (r-pad)%2==ph, (s-pad)%2==pw} dy[i-dh, j-dw] w[r,s]
-            for ph in range(2):
-                for pw in range(2):
-                    idx, tm, dw, dh = [], [], [], []
-                    for r in range(R):
-                        for s in range(S):
-                            oh, ow = r - pad, s - pad
-                            if oh % 2 == ph and ow % 2 == pw:
-                                idx.append(r * S + s)
-                                tm.append(0)
-                                dh.append(-((oh - ph) // 2))
-                                dw.append(-((ow - pw) // 2))
-                    out_view = dx[:, ph::2, pw::2, :]
-                    if not idx:
-                        self.needs_zero = True
-                        continue
-                    if wbufs is not None:
-                        wbuf = wbufs[len(self.parts)].view(len(idx) * cin, cout)
-                    else:
-                        wbuf = torch.empty(len(idx) * cin, cout, dtype=torch.bfloat16, device=dy.device)
-                        self._idx_dev[tuple(idx)] = torch.tensor(idx, device=dy.device, dtype=torch.long)
-                    box = pick_box(N, out_view.shape[1], out_view.shape[2])
-                    plan = ext.ConvPlan([dy], wbuf, out_view, tm, dw, dh, box[0], box[1], box[2], None, None, max_ctas)
-                    _plans.add(plan)
-                    self.parts.append((plan, wbuf, idx))
-                    self.boxes.append(box)
         self.refresh_weights()
 
     def refresh_weights(self) -> None:
@@ -292,26 +393,17 @@ class ConvWgrad:
 
     def __init__(self, dy: torch.Tensor, x: torch.Tensor, dw: torch.Tensor, R: int, S: int, stride: int = 1,
                  pad: int = 0, px_chunks: int = 0, max_ctas: int = 0, smem_budget: int = 0):
-        ext = _build.load("_b200_conv")
         taps = make_taps(x, R, S, stride, pad)
-        N, Ho, Wo, _ = dy.shape
+        N, Ho, Wo, cout = dy.shape
         flat = (R == 1 and S == 1 and stride == 1 and pad == 0 and x.is_contiguous() and dy.is_contiguous()
                 and (N * Ho * Wo) % 64 == 0)
-        if flat:
-            bw = bh = bn = 0
-        else:
-            # keep >= 3 pipeline stages in 227 KB: stage = (dY chunks + X chunks) * P pixels * 128 B (G <= 4 X chunks)
-            cin, cout = x.shape[3], dy.shape[3]
-            cb = cin // 64
-            g = S * (2 if (cb >= 2 and S * 2 <= 4) else 1) if S > 1 else max(d for d in (1, 2, 3, 4) if cb % d == 0)
-            chunks = (1 if cout == 64 else 2) + g
-            budget = smem_budget if 0 < smem_budget < 232448 else 232448
-            want_stages = 3 if budget >= 200000 else 2
-            rows = min(128, ((budget - 256 - 1024) // (want_stages * chunks * 128)) // 16 * 16)
-            bw, bh, bn = pick_box(N, Ho, Wo, rows=rows, multiple_of=16)
-        self.box = (bw, bh, bn)
-        self.plan = ext.WgradPlan(dy, taps.views, dw, R, S, taps.tap_map, taps.tap_dw, taps.tap_dh, bw, bh, bn,
-                                  px_chunks, max_ctas, smem_budget)
+        t = plan_wgrad(grid=(N, Ho, Wo), cin=x.shape[3], cout=cout, R=R, S=S, flat=flat, px_chunks=px_chunks,
+                       max_ctas=max_ctas, smem_budget=smem_budget, sm_count=sm_count())
+        self.box = t.box
+        bw, bh, bn = t.box
+        self.plan = _build.load("_b200_conv").WgradPlan(
+            dy, taps.views, dw, R, S, taps.tap_map, taps.tap_dw, taps.tap_dh, bw=bw, bh=bh, bn=bn,
+            cb_per_group=t.cb_per_group, stages=t.stages, px_chunks=t.px_chunks, grid=t.grid)
         _plans.add(self.plan)
 
     def run(self) -> None:

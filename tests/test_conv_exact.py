@@ -361,11 +361,15 @@ def test_conv_igemm_variant_coverage(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------ last-CTA tails
+TAIL_CASES = (ConvCase("tail_fwd", "fwd", 2, 16, 16, 64, 128, 1, 1, 1, 64, max_ctas=3, multi=True, env=_BN64),
+              ConvCase("tail_bwd", "dgrad", 2, 16, 16, 128, 64, 3, 1, 2, 64, max_ctas=5, multi=True, env=_BN64))
+
+
 def test_last_cta_tails_exact_sums(monkeypatch):
     """BatchNorm finalize / backward coefficients from the last CTA at max_ctas 3 / 5, run twice: the outputs equal the
     stand-alone kernels fed the exact sums, and the sums and the ticket counter are zero again after each run."""
     e = _ops()
-    fwd = ConvCase("tail_fwd", "fwd", 2, 16, 16, 64, 128, 1, 1, 1, 64, max_ctas=3, multi=True, env=_BN64)
+    fwd, bwd = TAIL_CASES
     d = _setup(fwd, monkeypatch, seed=5)
     plan, cout = d["plans"][0], fwd.cout
     g = torch.Generator(device=DEV).manual_seed(6)
@@ -391,7 +395,6 @@ def test_last_cta_tails_exact_sums(monkeypatch):
     for nm, a, b in zip(("mean", "invstd", "scale", "shift", "running_mean", "running_var"), outs + [rm, rv], ref + [rm2, rv2]):
         torch.testing.assert_close(a, b, rtol=1e-6, atol=1e-7, msg=lambda m, nm=nm: f"finalize {nm}: {m}")
 
-    bwd = ConvCase("tail_bwd", "dgrad", 2, 16, 16, 128, 64, 3, 1, 2, 64, max_ctas=5, multi=True, env=_BN64)
     d = _setup(bwd, monkeypatch, seed=7)
     cin = bwd.cin
     gam = torch.rand(cin, device=DEV, generator=g) + 0.5
@@ -460,8 +463,8 @@ WG_CASES = [
 ]
 
 
-@pytest.mark.parametrize("case", WG_CASES, ids=lambda c: c.id)
-def test_conv_wgrad_exact(case: WgCase):
+def _wgrad_op(case: WgCase):
+    """Builds the op of a wgrad case and its inputs: (op, x, dy, guarded dw)."""
     C = _C()
     g = torch.Generator(device=DEV).manual_seed(3)
     N, H, W, R, s = case.N, case.H, case.W, case.R, case.stride
@@ -472,6 +475,15 @@ def test_conv_wgrad_exact(case: WgCase):
     dw = Guarded((R * R * case.cout, case.cin), torch.float32, 0.0)
     op = C.ConvWgrad(dy, x, dw.t, R, R, s, pad, px_chunks=case.px_chunks, max_ctas=case.max_ctas,
                      smem_budget=case.smem_budget)
+    return op, x, dy, dw
+
+
+@pytest.mark.parametrize("case", WG_CASES, ids=lambda c: c.id)
+def test_conv_wgrad_exact(case: WgCase):
+    C = _C()
+    R, s = case.R, case.stride
+    pad = R // 2
+    op, x, dy, dw = _wgrad_op(case)
     p = op.plan
     assert (p.G, p.mode) == (case.G, case.mode)
     assert p.grid == min(p.units, case.max_ctas)

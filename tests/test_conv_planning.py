@@ -1,9 +1,12 @@
-"""CPU tests of the convolution planning layer (pixel boxes, tap tables, parity views) against torch conv semantics."""
+"""CPU tests of the convolution planning layer (pixel boxes, tap tables, parity views, tilings)."""
+import json
+
 import pytest
 import torch
 from hypothesis import given, settings, strategies as st
 
 from b200ddl.ops import conv as C
+from conv_plan_table import TABLE, WORKLOADS
 
 
 @settings(max_examples=60, deadline=None)
@@ -42,6 +45,26 @@ def test_tap_table_matches_conv2d(R, stride, pad, H):
     assert len(taps.views) <= 4
 
 
+@pytest.mark.parametrize("R,stride,pad,H", [(1, 1, 0, 6), (3, 1, 1, 6), (3, 2, 1, 8), (1, 2, 0, 8), (3, 2, 1, 14)])
+def test_dgrad_parity_parts_match_conv_transpose(R, stride, pad, H):
+    """The dgrad GEMMs (one per output-parity class, each a forward-style tap table over dy) sum to conv_transpose."""
+    torch.manual_seed(0)
+    Ho = (H + 2 * pad - R) // stride + 1
+    dy = torch.randn(2, Ho, Ho, 4)
+    w = torch.randn(R * R, 4, 5)   # [tap, Cout, Cin]
+    dx = torch.zeros(2, H, H, 5)
+    for (ph, pw), idx, dw, dh in C.ConvDgrad.parity_parts(R, R, stride, pad):
+        out = dx[:, ph::stride, pw::stride]
+        taps = C.TapTable([dy], [0] * len(idx), dw, dh)
+        out += _emulate(dy, taps, w[idx].transpose(1, 2), 1, 1, out.shape[1], out.shape[2])
+    ref = torch.nn.grad.conv2d_input((2, 5, H, H), C.weight_from_kernel_layout(w, R, R), dy.permute(0, 3, 1, 2),
+                                     stride=stride, padding=pad).permute(0, 2, 3, 1)
+    assert torch.allclose(dx, ref, atol=1e-4)
+    # the order the ResNet engine lays its dgrad weight copies out in
+    assert C.ConvDgrad.part_taps(3, 3, 2, 1) == [[4], [3, 5], [1, 7], [0, 2, 6, 8]]
+    assert C.ConvDgrad.part_taps(3, 3, 1, 1) == [list(range(9))]
+
+
 def test_weight_layout_roundtrip():
     w = torch.randn(8, 3, 3, 3)
     k = C.weight_to_kernel_layout(w)
@@ -65,19 +88,68 @@ def test_dgrad_refuses_fused_reductions_when_strided():
         C.ConvDgrad(dy, w, dx, 3, 3, 2, 1, block_grad=(dx, z, dx, z.clone(), z.clone()))
 
 
-def test_halo_box_selection(monkeypatch):
-    """Full-width single-image boxes only for the 3x3 / stride-1 / 64->64 layers whose box + halo fits one 28 KB stage and
-    whose width is a multiple of 8 (the vertical taps start whole 8-row swizzle atoms into the stage)."""
-    from b200ddl.ops import conv as C
+def _forward_tiling(h, w, cin=64, cout=64, R=3, stride=1, pad=1, switches=C.ConvSwitches()):
+    """plan_conv of a box-mode forward conv over a (2, h, w, cin) input (views and tap table from make_taps), and its
+    output grid."""
+    taps = C.make_taps(torch.empty(2, h, w, cin, device="meta"), R, R, stride, pad)
+    grid = (2, (h + 2 * pad - R) // stride + 1, (w + 2 * pad - R) // stride + 1)
+    t = C.plan_conv(grid=grid, view_widths=[v.shape[2] for v in taps.views], cin=cin, cout=cout, tap_map=taps.tap_map,
+                    tap_dw=taps.tap_dw, tap_dh=taps.tap_dh, flat=False, stats_mode=0, max_ctas=0, sm_count=132,
+                    switches=switches)
+    return t, grid
 
-    monkeypatch.delenv("B200DDL_NO_HALO", raising=False)
-    monkeypatch.delenv("B200DDL_NO_RESIDENT_FILTER", raising=False)
-    assert C.halo_box(56, 56, 64, 64, 3, 3, 1, 1) == (56, 2, 1)      # 112-pixel tile, 224-pixel halo stage
-    assert C.halo_box(24, 24, 64, 64, 3, 3, 1, 1) == (24, 4, 1)
-    assert C.halo_box(28, 28, 64, 64, 3, 3, 1, 1) is None            # 28-row tap offsets are not whole swizzle atoms
-    assert C.halo_box(56, 56, 128, 128, 3, 3, 1, 1) is None          # filter does not fit resident
-    assert C.halo_box(56, 56, 64, 64, 3, 3, 2, 1) is None            # strided
-    assert C.halo_box(56, 56, 64, 64, 1, 1, 1, 0) is None
-    assert C.halo_box(112, 112, 64, 64, 3, 3, 1, 1) is None          # one image row + halo exceeds a stage
+
+def test_halo_tiling_selection(monkeypatch):
+    """Full-width single-image boxes only for the 3x3 / stride-1 / 64->64 layers whose box + halo fits one 28 KB stage and
+    whose width is a multiple of 8 (the vertical taps start whole 8-row swizzle atoms into the stage); every other layer
+    gets the generic box."""
+    def halo(h, w, **kw):
+        t, grid = _forward_tiling(h, w, **kw)
+        if t.halo:
+            assert t.resident_filter
+            return t.box
+        assert t.box == C.pick_box(*grid)
+        return None
+
+    assert halo(56, 56) == (56, 2, 1)                    # 112-pixel tile, 224-pixel halo stage
+    assert halo(24, 24) == (24, 4, 1)
+    assert halo(28, 28) is None                          # 28-row tap offsets are not whole swizzle atoms
+    assert halo(56, 56, cin=128, cout=128) is None       # filter does not fit resident
+    assert halo(56, 56, stride=2) is None                # strided
+    assert halo(56, 56, R=1, pad=0) is None
+    assert halo(112, 112) is None                        # one image row + halo exceeds a stage
+    assert halo(56, 56, switches=C.ConvSwitches(no_halo=True)) is None
+    assert halo(56, 56, switches=C.ConvSwitches(no_resident_filter=True)) is None
+    for k in ("B200DDL_BLOCK_N", "B200DDL_NO_HALO", "B200DDL_NO_RESIDENT_FILTER"):
+        monkeypatch.delenv(k, raising=False)
+    assert C.conv_switches() == C.ConvSwitches()
     monkeypatch.setenv("B200DDL_NO_HALO", "1")
-    assert C.halo_box(56, 56, 64, 64, 3, 3, 1, 1) is None
+    monkeypatch.setenv("B200DDL_BLOCK_N", "128")
+    assert C.conv_switches() == C.ConvSwitches(block_n=128, no_halo=True)
+    monkeypatch.setenv("B200DDL_NO_RESIDENT_FILTER", "1")
+    monkeypatch.setenv("B200DDL_BLOCK_N", "96")
+    assert C.conv_switches() == C.ConvSwitches(no_halo=True, no_resident_filter=True)
+
+
+def test_planner_reproduces_recorded_plans():
+    """Every plan of the flagship workloads and of the bit-exact kernel cases (tests/golden/conv_plans.json, recorded on
+    an H100), replayed through the pure planner: the same tiling, field for field."""
+    with open(TABLE) as f:
+        table = json.load(f)
+    sm = table["sm_count"]
+    seen = set()
+    for i, op in enumerate(table["ops"]):
+        for j, p in enumerate(op["plans"]):
+            inp, want = dict(p["inputs"]), p["props"]
+            if op["op"] == "ConvWgrad":
+                t = C.plan_wgrad(**inp, sm_count=sm)
+                got = dict(grid=t.grid, units=t.units, stages=t.stages, G=t.G, px_chunks=t.px_chunks,
+                           mode=int(not inp["flat"]))
+            else:
+                inp["switches"] = C.ConvSwitches(**inp["switches"])
+                t = C.plan_conv(**inp, sm_count=sm)
+                got = dict(block_n=t.block_n, resident_filter=int(t.resident_filter), halo=int(t.halo), tiles=t.tiles,
+                           grid=t.grid, stats_mode=inp["stats_mode"], has_tail=False)
+            assert (list(t.box), got) == (p["box"], want), f"op {i} ({op['workload']} {op['op']}) plan {j}: {inp}"
+            seen.add(op["workload"])
+    assert seen == set(WORKLOADS)
