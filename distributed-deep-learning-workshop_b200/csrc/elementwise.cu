@@ -132,14 +132,14 @@ __device__ __forceinline__ void bn_bwd_coeffs8(const BnBwdFuse& f, int c0, bool 
 }
 
 // ------------------------------------------------------------------------------------------------ BN apply
-// out = [relu]( y*scale + shift  [+ res | + res*res_scale + res_shift] )
+// out = act( y*scale + shift  [+ res | + res*res_scale + res_shift] ),  act: identity, ReLU or ReLU6 (ACT 0 / 1 / 2)
 // Column-resident: a thread owns one 8-channel column vector and walks down the rows, so the per-channel
 // parameters are loaded into registers once instead of once per element (L1 traffic was 5x the payload).
 // U: rows per loop iteration.  All loads of the U rows are issued before the first is consumed: with one row per iteration a
 // thread has one or two 16-byte loads in flight and the kernel sits at ~64 % of the measured copy bandwidth (ncu: bn_bwd_apply
 // 4.2 of 6.57 TB/s at 34 % occupancy - too few bytes in flight for HBM3e's latency); the per-element arithmetic and its order
 // are unchanged, so every U produces bit-identical results.
-template <bool RELU, int RES, bool FUSED = false, int U = 1>  // RES: 0 none, 1 identity residual, 2 residual with its own BN
+template <int ACT, int RES, bool FUSED = false, int U = 1>  // RES: 0 none, 1 identity residual, 2 residual with its own BN
 __global__ void __launch_bounds__(256, U > 1 ? 3 : 1)
 bn_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ scale,
                 const float* __restrict__ shift, const __nv_bfloat16* __restrict__ res,
@@ -196,7 +196,7 @@ bn_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ s
 #pragma unroll
         for (int k = 0; k < 8; ++k) f[k] += q[k];
       }
-      if (RELU) {
+      if (ACT == 1) {
         if (mask != nullptr) {  // 1 bit per element: the backward pass reads this instead of the activation
           uint32_t mbits = 0;
 #pragma unroll
@@ -205,6 +205,9 @@ bn_apply_kernel(const __nv_bfloat16* __restrict__ y, const float* __restrict__ s
         }
 #pragma unroll
         for (int k = 0; k < 8; ++k) f[k] = fmaxf(f[k], 0.f);
+      } else if (ACT == 2) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) f[k] = fminf(fmaxf(f[k], 0.f), 6.f);
       }
       st8(out + off, pack8(f));
       }
@@ -232,7 +235,7 @@ static inline int rows_grid(int64_t M, int C, int threads) {
 }
 
 void bn_apply(const void* y, const float* scale, const float* shift, const void* res, const float* res_scale,
-              const float* res_shift, void* out, void* mask, int64_t M, int C, bool relu, cudaStream_t s) {
+              const float* res_shift, void* out, void* mask, int64_t M, int C, int act, cudaStream_t s) {
   const int threads = 256;
   const int blocks = rows_grid(M, C, threads);
   auto Y = (const __nv_bfloat16*)y;
@@ -249,10 +252,12 @@ void bn_apply(const void* y, const float* scale, const float* shift, const void*
     else                                                                                                             \
       bn_apply_kernel<RL, RM><<<blocks, threads, 0, s>>>(Y, scale, shift, R, res_scale, res_shift, O, MK, M, C);     \
   } while (0)
-  if (relu) {
-    if (rmode == 0) LAUNCH(true, 0); else if (rmode == 1) LAUNCH(true, 1); else LAUNCH(true, 2);
+  if (act == 1) {
+    if (rmode == 0) LAUNCH(1, 0); else if (rmode == 1) LAUNCH(1, 1); else LAUNCH(1, 2);
+  } else if (act == 2) {   // ReLU6 (MobileNetV2 training-mode BatchNorm): no second BatchNorm on the residual
+    if (rmode == 0) LAUNCH(2, 0); else LAUNCH(2, 1);
   } else {
-    if (rmode == 0) LAUNCH(false, 0); else if (rmode == 1) LAUNCH(false, 1); else LAUNCH(false, 2);
+    if (rmode == 0) LAUNCH(0, 0); else if (rmode == 1) LAUNCH(0, 1); else LAUNCH(0, 2);
   }
 #undef LAUNCH
 }
@@ -269,9 +274,9 @@ void bn_apply_fused(const void* y, const BnFwdFuse& f, const void* res, const Bn
   const BnFwdFuse rz = res_f != nullptr ? *res_f : BnFwdFuse();
 #define LAUNCH(RL, RM) bn_apply_kernel<RL, RM, true><<<blocks, threads, 0, s>>>(Y, nullptr, nullptr, R, nullptr, nullptr, O, MK, M, C, f, rz)
   if (relu) {
-    if (rmode == 0) LAUNCH(true, 0); else if (rmode == 1) LAUNCH(true, 1); else LAUNCH(true, 2);
+    if (rmode == 0) LAUNCH(1, 0); else if (rmode == 1) LAUNCH(1, 1); else LAUNCH(1, 2);
   } else {
-    if (rmode == 0) LAUNCH(false, 0); else if (rmode == 1) LAUNCH(false, 1); else LAUNCH(false, 2);
+    if (rmode == 0) LAUNCH(0, 0); else if (rmode == 1) LAUNCH(0, 1); else LAUNCH(0, 2);
   }
 #undef LAUNCH
 }

@@ -1,5 +1,6 @@
-// Backward kernels of MobileNetV2 fine-tuning with the base's BatchNorm in inference mode (models/mobilenet_engine.py,
-// `fine_tune_at`).  A trainable layer computes c = conv(x, W), z = s*c + t with the folded affine s = gamma*invstd,
+// Backward kernels of MobileNetV2 fine-tuning (models/mobilenet_engine.py, `fine_tune_at`).  With the base's BatchNorm in
+// inference mode (below); with training-mode BatchNorm the engine combines relu6_mask_reduce (also summing dz * c) and the
+// depthwise / stem kernels here with the ResNet-50 BatchNorm kernels of elementwise.cu (DESIGN.md 3.5b).  A trainable layer computes c = conv(x, W), z = s*c + t with the folded affine s = gamma*invstd,
 // t = beta - mean*s (frozen statistics), and y = act(z [+ residual]).  With g the gradient arriving at y:
 //
 //   dz = g * [0 < y < 6]  (ReLU6, mask from the stored bf16 y)   or   dz = g1 + g2  (linear project layer + skip)
@@ -58,16 +59,19 @@ constexpr int kTW = 4;   // output (wgrad) / input (dgrad) pixels per thread alo
 // ------------------------------------------------------------------------------------------------ ReLU6 mask + reduction
 // Block = 8 channel vectors (64 channels, blockIdx.x) x 32 row lanes; rows grid-stride over blockIdx.y.
 // dz may alias g1 (element-wise, each element read before it is written by the same thread).
-template <bool RELU6, bool G2>
+// DZC (training-mode BatchNorm): also sum_dzc[ch] += sum(dz * c) with c the stored bf16 conv output, the same lanes and
+// the same fixed in-CTA order as sum(dz).
+template <bool RELU6, bool G2, bool DZC = false>
 __global__ void __launch_bounds__(256)
 relu6_mask_reduce_kernel(const __nv_bfloat16* g1, const __nv_bfloat16* __restrict__ g2, const __nv_bfloat16* __restrict__ y,
-                         __nv_bfloat16* dz, float* __restrict__ sum, int64_t M, int C) {
-  __shared__ float red[8][64];
+                         __nv_bfloat16* dz, float* __restrict__ sum, int64_t M, int C,
+                         const __nv_bfloat16* __restrict__ cin = nullptr, float* __restrict__ sum_dzc = nullptr) {
+  __shared__ float red[DZC ? 2 : 1][8][64];
   const int cv = blockIdx.x * 8 + (threadIdx.x & 7);
   const bool active = cv < C / 8;
-  float acc[8];
+  float acc[8], acc2[8];
 #pragma unroll
-  for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+  for (int k = 0; k < 8; ++k) acc[k] = acc2[k] = 0.f;
   if (active) {
     for (int64_t m = blockIdx.y * 32 + (threadIdx.x >> 3); m < M; m += (int64_t)gridDim.y * 32) {
       const int64_t o = m * C + cv * 8;
@@ -90,17 +94,30 @@ relu6_mask_reduce_kernel(const __nv_bfloat16* g1, const __nv_bfloat16* __restric
       unpack(d, g);   // sum the stored (bf16) gradient
 #pragma unroll
       for (int k = 0; k < 8; ++k) acc[k] += g[k];
+      if (DZC) {
+        float cc[8];
+        unpack(*reinterpret_cast<const bfx8*>(cin + o), cc);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc2[k] = fmaf(g[k], cc[k], acc2[k]);
+      }
     }
   }
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], 8);
     acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], 16);
+    if (DZC) {
+      acc2[k] += __shfl_xor_sync(0xffffffffu, acc2[k], 8);
+      acc2[k] += __shfl_xor_sync(0xffffffffu, acc2[k], 16);
+    }
   }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (lane < 8) {
 #pragma unroll
-    for (int k = 0; k < 8; ++k) red[warp][lane * 8 + k] = acc[k];
+    for (int k = 0; k < 8; ++k) {
+      red[0][warp][lane * 8 + k] = acc[k];
+      if (DZC) red[DZC ? 1 : 0][warp][lane * 8 + k] = acc2[k];
+    }
   }
   __syncthreads();
   if (threadIdx.x < 64) {
@@ -108,13 +125,19 @@ relu6_mask_reduce_kernel(const __nv_bfloat16* g1, const __nv_bfloat16* __restric
     if (c < C) {
       float s = 0.f;
 #pragma unroll
-      for (int w = 0; w < 8; ++w) s += red[w][threadIdx.x];
+      for (int w = 0; w < 8; ++w) s += red[0][w][threadIdx.x];
       atomicAdd(sum + c, s);
+      if (DZC) {
+        float s2 = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) s2 += red[DZC ? 1 : 0][w][threadIdx.x];
+        atomicAdd(sum_dzc + c, s2);
+      }
     }
   }
 }
-void relu6_mask_reduce(const void* g1, const void* g2, const void* y, void* dz, float* sum, int64_t M, int C, bool relu6,
-                       cudaStream_t s) {
+void relu6_mask_reduce(const void* g1, const void* g2, const void* y, void* dz, float* sum, const void* c, float* sum_dzc,
+                       int64_t M, int C, bool relu6, cudaStream_t s) {
   const int gx = (C / 8 + 7) / 8;
   const int gy = blocks_for(M, 32, (132 * 8 + gx - 1) / gx);
   const dim3 grid(gx, gy);
@@ -122,6 +145,14 @@ void relu6_mask_reduce(const void* g1, const void* g2, const void* y, void* dz, 
   auto b = (const __nv_bfloat16*)g2;
   auto v = (const __nv_bfloat16*)y;
   auto d = (__nv_bfloat16*)dz;
+  if (c != nullptr) {   // training-mode BatchNorm: ReLU6 layers have no skip gradient, linear layers may have one
+    auto cc = (const __nv_bfloat16*)c;
+    if (relu6 && g2)      relu6_mask_reduce_kernel<true, true, true><<<grid, 256, 0, s>>>(a, b, v, d, sum, M, C, cc, sum_dzc);
+    else if (relu6)       relu6_mask_reduce_kernel<true, false, true><<<grid, 256, 0, s>>>(a, b, v, d, sum, M, C, cc, sum_dzc);
+    else if (g2)          relu6_mask_reduce_kernel<false, true, true><<<grid, 256, 0, s>>>(a, b, v, d, sum, M, C, cc, sum_dzc);
+    else                  relu6_mask_reduce_kernel<false, false, true><<<grid, 256, 0, s>>>(a, b, v, d, sum, M, C, cc, sum_dzc);
+    return;
+  }
   if (relu6 && g2)        relu6_mask_reduce_kernel<true, true><<<grid, 256, 0, s>>>(a, b, v, d, sum, M, C);
   else if (relu6)         relu6_mask_reduce_kernel<true, false><<<grid, 256, 0, s>>>(a, b, v, d, sum, M, C);
   else if (g2)            relu6_mask_reduce_kernel<false, true><<<grid, 256, 0, s>>>(a, b, v, d, sum, M, C);

@@ -41,7 +41,7 @@ void bn_finalize(float* sum, float* sqsum, double count, const float* gamma, con
 void set_bn_rows_unroll(int u);
 int get_bn_rows_unroll();
 void bn_apply(const void* y, const float* scale, const float* shift, const void* res, const float* res_scale,
-              const float* res_shift, void* out, void* mask, int64_t M, int C, bool relu, cudaStream_t s);
+              const float* res_shift, void* out, void* mask, int64_t M, int C, int act, cudaStream_t s);
 void channel_stats(const void* y, float* sum, float* sqsum, int64_t M, int C, cudaStream_t s);
 void bn_bwd_reduce(int mode, const void* g1, const void* g2, const void* outp, const void* y, const float* scale,
                    const float* shift, void* dz_out, float* sum_dz, float* sum_dzy, int64_t M, int C, cudaStream_t s);
@@ -69,6 +69,12 @@ void mbv2_stem(const uint8_t* x, const float* w, const float* scale, const float
                int ldc, float mul, float add, cudaStream_t s);
 void dwconv3x3(const void* x, const float* w, const float* scale, const float* shift, void* out, int N, int H, int W, int C,
                int stride, int tile_w, cudaStream_t s);
+// Training-mode BatchNorm variants: c = conv(x) stored as bf16, no affine / clamp, and sum[c] += sum(c), sqsum[c] +=
+// sum(c^2) of the stored (bf16) values (zeroed by the caller).  mbv2_stem_stats writes and sums the 32 real channels.
+void mbv2_stem_stats(const uint8_t* x, const float* w, void* out, float* sum, float* sqsum, int N, int H, int W, int ldc,
+                     float mul, float add, cudaStream_t s);
+void dwconv3x3_stats(const void* x, const float* w, void* out, float* sum, float* sqsum, int N, int H, int W, int C,
+                     int stride, int tile_w, cudaStream_t s);
 void preprocess_u8(const uint8_t* x, void* out, int64_t npix, int cpad, float mul, float add, cudaStream_t s);
 void resize_bilinear_u8(const uint8_t* x, uint8_t* out, int N, int H, int W, int OH, int OW, bool planar, cudaStream_t s);
 void weight_prep(const float* w, void* wf, void* wd, int taps, int cout, int cin, cudaStream_t s);
@@ -116,9 +122,10 @@ void lamb_apply(float* p, const float* m, const float* v, void* p16, int64_t n, 
                 int64_t nchunks, const float* phi, int nseg, const float* hyper, cudaStream_t s);
 void cast_f32_to_bf16(const float* x, void* out, int64_t n, cudaStream_t s);
 
-// MobileNetV2 fine-tuning backward with inference-mode BatchNorm (csrc/mobilenet_bwd.cu).
-void relu6_mask_reduce(const void* g1, const void* g2, const void* y, void* dz, float* sum, int64_t M, int C, bool relu6,
-                       cudaStream_t s);
+// MobileNetV2 fine-tuning backward (csrc/mobilenet_bwd.cu).  relu6_mask_reduce: with c (training-mode BatchNorm, the
+// conv output before normalisation) it also accumulates sum_dzc[ch] += sum(dz * c).
+void relu6_mask_reduce(const void* g1, const void* g2, const void* y, void* dz, float* sum, const void* c, float* sum_dzc,
+                       int64_t M, int C, bool relu6, cudaStream_t s);
 void dw_dgrad(const void* dz, const float* w, const float* scale, void* dx, int N, int H, int W, int C, int stride,
               cudaStream_t s);
 void dw_wgrad(const void* dz, const void* x, float* G, int N, int H, int W, int C, int stride, cudaStream_t s);

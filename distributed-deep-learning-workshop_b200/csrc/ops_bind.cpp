@@ -65,8 +65,11 @@ inline void same_act(const Tensor& t, const Tensor& like, const char* name) {
   aligned(t, 16, name);
 }
 
+// relu6: cap the ReLU at 6 (needs relu; no ReLU bitmask, no BatchNorm on the residual)
 void bn_apply(Tensor y, Tensor scale, Tensor shift, OptT res, OptT res_scale, OptT res_shift, Tensor out, bool relu,
-              OptT mask) {
+              OptT mask, bool relu6) {
+  TORCH_CHECK(!relu6 || (relu && !mask.has_value() && !res_scale.has_value()),
+              "relu6 caps the ReLU: it needs relu=True, and takes no mask and no res_scale / res_shift");
   const int C = act_channels(y, "y");
   const int64_t M = y.numel() / C;
   same_act(out, y, "out");
@@ -78,7 +81,8 @@ void bn_apply(Tensor y, Tensor scale, Tensor shift, OptT res, OptT res_scale, Op
   if (res_scale.has_value()) { vec(*res_scale, at::kFloat, C, "res_scale"); vec(*res_shift, at::kFloat, C, "res_shift"); }
   if (mask.has_value()) { chk(*mask, at::kByte, "mask"); TORCH_CHECK(mask->numel() * 8 == y.numel()); }
   b200::bn_apply(y.data_ptr(), scale.data_ptr<float>(), shift.data_ptr<float>(), vp(res), fp(res_scale),
-                 fp(res_shift), out.data_ptr(), mask.has_value() ? mask->data_ptr() : nullptr, M, C, relu, cur());
+                 fp(res_shift), out.data_ptr(), mask.has_value() ? mask->data_ptr() : nullptr, M, C,
+                 relu6 ? 2 : (relu ? 1 : 0), cur());
   after();
 }
 
@@ -376,6 +380,43 @@ void dwconv3x3(Tensor x, Tensor w, Tensor scale, Tensor shift, Tensor out, int64
                   (int)x.size(0), H, W, C, (int)stride, (int)tile_w, cur());
   after();
 }
+// NHWC bf16 pair of a depthwise 3x3 (pad 1) layer: input grid x, output grid (H-1)/stride+1; returns C
+static int dw_pair(const Tensor& x, const Tensor& dz, int64_t stride, const char* xname) {
+  TORCH_CHECK(stride == 1 || stride == 2, "stride must be 1 or 2");
+  TORCH_CHECK(x.dim() == 4 && dz.dim() == 4, "depthwise operands are NHWC");
+  const int C = act_channels(x, xname);
+  act_channels(dz, "dz");
+  TORCH_CHECK(dz.size(0) == x.size(0) && dz.size(3) == C && dz.size(1) == (x.size(1) - 1) / stride + 1 &&
+              dz.size(2) == (x.size(2) - 1) / stride + 1, "dz shape does not match the input grid and stride");
+  return C;
+}
+// training-mode BatchNorm variants: c = conv (bf16, no affine / clamp) and sum / sqsum += per-channel sum(c), sum(c^2)
+// of the stored values (zeroed by the caller)
+void mbv2_stem_stats(Tensor x, Tensor w, Tensor out, Tensor sum, Tensor sqsum, double mul, double add) {
+  chk(x, at::kByte, "x");
+  TORCH_CHECK(x.dim() == 4 && x.size(3) == 3 && x.size(1) % 2 == 0 && x.size(2) % 2 == 0,
+              "stem input: uint8 [N, H, W, 3], even H / W");
+  vec(w, at::kFloat, 27 * 32, "w", 4);
+  const int ldc = act_channels(out, "out");
+  TORCH_CHECK(out.dim() == 4 && out.size(0) == x.size(0) && out.size(1) == x.size(1) / 2 && out.size(2) == x.size(2) / 2 &&
+              ldc >= 32, "out: bf16 [N, H/2, W/2, ldc >= 32]");
+  vec(sum, at::kFloat, 32, "sum", 1);
+  vec(sqsum, at::kFloat, 32, "sqsum", 1);
+  b200::mbv2_stem_stats(x.data_ptr<uint8_t>(), w.data_ptr<float>(), out.data_ptr(), sum.data_ptr<float>(),
+                        sqsum.data_ptr<float>(), (int)x.size(0), (int)x.size(1), (int)x.size(2), ldc, (float)mul,
+                        (float)add, cur());
+  after();
+}
+void dwconv3x3_stats(Tensor x, Tensor w, Tensor out, Tensor sum, Tensor sqsum, int64_t stride, int64_t tile_w) {
+  TORCH_CHECK(tile_w == 1 || tile_w == 4, "tile_w must be 1 or 4");
+  const int C = dw_pair(x, out, stride, "x");
+  vec(w, at::kFloat, 9 * (int64_t)C, "w");
+  vec(sum, at::kFloat, C, "sum", 1);
+  vec(sqsum, at::kFloat, C, "sqsum", 1);
+  b200::dwconv3x3_stats(x.data_ptr(), w.data_ptr<float>(), out.data_ptr(), sum.data_ptr<float>(), sqsum.data_ptr<float>(),
+                        (int)x.size(0), (int)x.size(1), (int)x.size(2), C, (int)stride, (int)tile_w, cur());
+  after();
+}
 void preprocess_u8(Tensor x, Tensor out, double mul, double add) {
   chk(x, at::kByte, "x");
   chk(out, at::kBFloat16, "out");
@@ -567,25 +608,22 @@ void cast_bf16(Tensor x, Tensor out) {
 
 // ------------------------------------------------------------------------------------------------ MobileNetV2 fine-tuning
 // dz = g1 [+ g2], masked by 0 < y < 6 when relu6; sum[c] += sum_rows dz (sum must be zeroed by the caller).  dz may be g1.
-void relu6_mask_reduce(Tensor g1, OptT g2, Tensor y, Tensor dz, Tensor sum, bool relu6) {
+// With c (bf16, y's shape; training-mode BatchNorm) also sum_dzc[ch] += sum_rows dz * c; c and sum_dzc go together.
+void relu6_mask_reduce(Tensor g1, OptT g2, Tensor y, Tensor dz, Tensor sum, bool relu6, OptT c, OptT sum_dzc) {
   const int C = act_channels(y, "y");
   same_act(g1, y, "g1");
   same_act(dz, y, "dz");
   if (g2.has_value()) same_act(*g2, y, "g2");
   vec(sum, at::kFloat, C, "sum", 1);
-  b200::relu6_mask_reduce(g1.data_ptr(), vp(g2), y.data_ptr(), dz.data_ptr(), sum.data_ptr<float>(), y.numel() / C, C,
-                          relu6, cur());
+  TORCH_CHECK(c.has_value() == sum_dzc.has_value(), "c and sum_dzc go together");
+  if (c.has_value()) {
+    same_act(*c, y, "c");
+    vec(*sum_dzc, at::kFloat, C, "sum_dzc", 1);
+    TORCH_CHECK(c->data_ptr() != dz.data_ptr(), "dz must not overwrite c");
+  }
+  b200::relu6_mask_reduce(g1.data_ptr(), vp(g2), y.data_ptr(), dz.data_ptr(), sum.data_ptr<float>(), vp(c),
+                          sum_dzc.has_value() ? sum_dzc->data_ptr<float>() : nullptr, y.numel() / C, C, relu6, cur());
   after();
-}
-// NHWC bf16 pair of a depthwise 3x3 (pad 1) layer: input grid x, output grid (H-1)/stride+1; returns C
-static int dw_pair(const Tensor& x, const Tensor& dz, int64_t stride, const char* xname) {
-  TORCH_CHECK(stride == 1 || stride == 2, "stride must be 1 or 2");
-  TORCH_CHECK(x.dim() == 4 && dz.dim() == 4, "depthwise operands are NHWC");
-  const int C = act_channels(x, xname);
-  act_channels(dz, "dz");
-  TORCH_CHECK(dz.size(0) == x.size(0) && dz.size(3) == C && dz.size(1) == (x.size(1) - 1) / stride + 1 &&
-              dz.size(2) == (x.size(2) - 1) / stride + 1, "dz shape does not match the input grid and stride");
-  return C;
 }
 // dx = conv_transpose(dz, scale (.) w) of a depthwise 3x3;  w fp32 [9, C], scale fp32 [C]
 void dw_dgrad(Tensor dz, Tensor w, Tensor scale, Tensor dx, int64_t stride) {
@@ -698,7 +736,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("bn_finalize", &bn_finalize);
   m.def("bn_apply", &bn_apply, py::arg("y"), py::arg("scale"), py::arg("shift"), py::arg("res") = c10::nullopt,
         py::arg("res_scale") = c10::nullopt, py::arg("res_shift") = c10::nullopt, py::arg("out"), py::arg("relu") = true,
-        py::arg("mask") = c10::nullopt);
+        py::arg("mask") = c10::nullopt, py::arg("relu6") = false);
   m.def("channel_stats", &channel_stats);
   m.def("bn_bwd_reduce", &bn_bwd_reduce);
   m.def("bn_bwd_coeffs", &bn_bwd_coeffs);
@@ -727,6 +765,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mbv2_stem", &mbv2_stem);
   m.def("dwconv3x3", &dwconv3x3, pybind11::arg("x"), pybind11::arg("w"), pybind11::arg("scale"), pybind11::arg("shift"),
         pybind11::arg("out"), pybind11::arg("stride"), pybind11::arg("tile_w") = 4);
+  m.def("mbv2_stem_stats", &mbv2_stem_stats, py::arg("x"), py::arg("w"), py::arg("out"), py::arg("sum"), py::arg("sqsum"),
+        py::arg("mul"), py::arg("add"));
+  m.def("dwconv3x3_stats", &dwconv3x3_stats, py::arg("x"), py::arg("w"), py::arg("out"), py::arg("sum"), py::arg("sqsum"),
+        py::arg("stride"), py::arg("tile_w") = 4);
   m.def("preprocess_u8", &preprocess_u8);
   m.def("resize_bilinear_u8", &resize_bilinear_u8, py::arg("x"), py::arg("out"), py::arg("planar") = false);
   m.def("weight_prep", &weight_prep);
@@ -748,7 +790,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("launch_count", [] { return g_launches; });
   m.def("reset_launch_count", [] { g_launches = 0; });
   m.def("relu6_mask_reduce", &relu6_mask_reduce, py::arg("g1"), py::arg("g2"), py::arg("y"), py::arg("dz"), py::arg("sum"),
-        py::arg("relu6") = true);
+        py::arg("relu6") = true, py::arg("c") = c10::nullopt, py::arg("sum_dzc") = c10::nullopt);
   m.def("dw_dgrad", &dw_dgrad);
   m.def("dw_wgrad", &dw_wgrad);
   m.def("mbv2_stem_wgrad", &mbv2_stem_wgrad);

@@ -25,7 +25,7 @@ CLASSES = ["daisy", "dandelion", "roses", "sunflowers", "tulips"]  # reference P
 def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_channels: int = IMG_CHANNELS,
                 num_classes: int = 5, dropout: float = 0.5, arch: Optional[str] = None, batch_size: int = 32,
                 freeze_base: bool = True, device=None, seed: int = 0, fine_tune_at: Optional[int] = None,
-                augmentation: Optional[Augmentation] = None, **engine_kwargs):
+                augmentation: Optional[Augmentation] = None, batchnorm: str = "inference", **engine_kwargs):
     """``fine_tune_at=k`` (MobileNetV2 only, 0..19) fine-tunes ``base.features[k:]`` - conv weights and BatchNorm
     weight / bias - with every BatchNorm of the base in inference mode (Keras's ``base_model(x, training=False)``).
     ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only), not
@@ -34,12 +34,21 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
 
     ``augmentation`` (`Augmentation`): random flip / rotation / zoom / translation of every training batch (Keras's
     augmentation layers in front of the model), on the device for the native engines; ``evaluate`` / ``predict`` never
-    augment.  ``None`` (default) leaves every path unchanged.  Not available for ``arch='resnet50_torch'``."""
+    augment.  ``None`` (default) leaves every path unchanged.  Not available for ``arch='resnet50_torch'``.
+
+    ``batchnorm`` (MobileNetV2 with ``fine_tune_at`` only): ``"inference"`` (default) as above, or ``"training"`` - the
+    BatchNorms of ``base.features[k:]`` normalise with batch statistics in training steps and update their running
+    statistics; ``evaluate`` / ``predict`` use the running statistics."""
     if isinstance(img_height, float) and img_width == IMG_WIDTH:  # build_model(dropout) positional form
         dropout, img_height = img_height, IMG_HEIGHT
     if img_channels != 3:
         raise ValueError("only 3-channel images are supported")
     augmentation = check_augmentation(augmentation)
+    from .mobilenet import check_batchnorm
+
+    check_batchnorm(batchnorm, fine_tune_at)
+    if batchnorm == "training" and arch in ("resnet50", "resnet50_torch"):
+        raise ValueError("batchnorm='training' applies to the MobileNetV2 model only")
     if fine_tune_at is not None:
         from .mobilenet import check_fine_tune_at
 
@@ -63,7 +72,8 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
         from .mobilenet_engine import MobileNetV2Engine
 
         return MobileNetV2Engine(batch=batch_size, num_classes=num_classes, device=device, image_size=img_height,
-                                 dropout=dropout, seed=seed, fine_tune_at=fine_tune_at, augmentation=augmentation)
+                                 dropout=dropout, seed=seed, fine_tune_at=fine_tune_at, augmentation=augmentation,
+                                 batchnorm=batchnorm)
     if arch in ("mobilenetv2", "mobilenetv2_torch"):
         from .mobilenet import FrozenBaseClassifier, MobileNetV2Base
 
@@ -72,7 +82,7 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
             torch.manual_seed(seed)
             base = MobileNetV2Base()
             return FrozenBaseClassifier(base, base.out_channels, num_classes, dropout, freeze_base, fine_tune_at,
-                                        augmentation=augmentation, augmentation_seed=seed)
+                                        augmentation=augmentation, augmentation_seed=seed, batchnorm=batchnorm)
     if arch == "resnet50_torch":
         if augmentation is not None:
             raise ValueError("arch='resnet50_torch' is the plain torchvision module and takes no augmentation")

@@ -68,6 +68,19 @@ def check_fine_tune_at(fine_tune_at, freeze_base: bool = True) -> None:
         raise ValueError(f"fine_tune_at must be an int in 0..{NUM_FEATURE_BLOCKS}, got {fine_tune_at!r}")
 
 
+BATCHNORM_MODES = ("inference", "training")
+
+
+def check_batchnorm(batchnorm, fine_tune_at) -> None:
+    """``batchnorm="training"`` normalises the trainable blocks ``base.features[fine_tune_at:]`` with batch statistics;
+    it needs ``fine_tune_at`` (the whole base in training mode is ``freeze_base=False``)."""
+    if batchnorm not in BATCHNORM_MODES:
+        raise ValueError(f"batchnorm must be 'inference' or 'training', got {batchnorm!r}")
+    if batchnorm == "training" and fine_tune_at is None:
+        raise ValueError("batchnorm='training' applies to the trainable blocks of fine_tune_at=k; to train the whole "
+                         "base with training-mode BatchNorm pass freeze_base=False instead")
+
+
 class FrozenBaseClassifier(nn.Module):
     """Sequential[base (frozen, inference-mode BN), GlobalAveragePooling2D, Dropout(p), Dense(num_classes)] - logits.
 
@@ -77,16 +90,23 @@ class FrozenBaseClassifier(nn.Module):
     ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only), not
     Keras's 154 ``base_model.layers``.
 
+    ``batchnorm="training"`` (with ``fine_tune_at=k``) puts the BatchNorms of ``base.features[k:]`` in training mode in
+    ``train()``: batch statistics, running statistics updated (momentum 0.1, eps 1e-5), as Keras does when the top of
+    ``base_model`` is unfrozen and called without ``training=False``.  ``features[:k]`` stay in inference mode.
+
     ``augmentation`` (`models.augment.Augmentation`) is applied by the trainer's module backend to the uint8 batch of
     every training step (the reference implementation of the engines' kernels, keyed by ``augmentation_seed`` and the
     rank); the module's own forward never augments."""
 
     def __init__(self, base: nn.Module, feat_channels: int, num_classes: int, dropout: float = 0.5,
-                 freeze_base: bool = True, fine_tune_at=None, augmentation=None, augmentation_seed: int = 0):
+                 freeze_base: bool = True, fine_tune_at=None, augmentation=None, augmentation_seed: int = 0,
+                 batchnorm: str = "inference"):
         from .augment import check_augmentation
 
         super().__init__()
         check_fine_tune_at(fine_tune_at, freeze_base)
+        check_batchnorm(batchnorm, fine_tune_at)
+        self.batchnorm = batchnorm
         self.augmentation = check_augmentation(augmentation)
         self.augmentation_seed = int(augmentation_seed)
         self.base = base
@@ -105,6 +125,8 @@ class FrozenBaseClassifier(nn.Module):
         super().train(mode)
         if self.freeze_base:
             self.base.eval()  # frozen base => BatchNorm in inference mode (Keras `layer.trainable = False`)
+            if self.batchnorm == "training":
+                self.base.features[self.fine_tune_at:].train(mode)
         return self
 
     def forward(self, x):

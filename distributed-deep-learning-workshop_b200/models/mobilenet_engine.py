@@ -24,6 +24,16 @@ then turns G into dW = scale * G, dgamma = invstd * (<W_c, G_c> - mean * dbeta),
 in the flat buffers in backward-completion order (fc, then features.18 down to features.k), each in the layout its
 kernel reads: pointwise [cout_p, cin_p] (zero padding, which gets zero gradient), depthwise [9, Cp], stem [27, 32],
 gamma / beta [c].  The running statistics stay outside the buffers and never change.
+
+``batchnorm="training"`` (with ``fine_tune_at=k <= 18``) normalises the trainable layers with batch statistics in
+training steps (DESIGN.md 3.5b): c = conv(x) is stored (bf16) with its per-channel sums (the kStats = 1 GEMM epilogue, or
+the statistics variants of the depthwise / stem kernels), bn_finalize turns them into the batch affine and updates the
+running statistics, bn_apply writes y = act(affine(c) [+ residual]).  Backward per layer: dz with sum(dz), sum(dz*c)
+(relu6_mask_reduce), bn_bwd_coeffs (dgamma / dbeta straight into the flat gradient buffer), dc = A*dz + B*c + C
+(bn_bwd_apply), then the weight and data gradients of dc with the plain filter.  After the optimizer,
+refresh_derived_weights folds the running statistics into the inference affine (bn_finalize in inference mode) that
+evaluation uses, and rebuilds the plain bf16 dgrad filters.  The running statistics of the trainable layers live in
+``running`` (means, then variances); frozen layers and evaluation keep the launches above.
 """
 from __future__ import annotations
 
@@ -50,13 +60,16 @@ class MobileNetV2Engine:
 
     def __init__(self, batch: int, num_classes: int = 5, device: Optional[torch.device] = None, image_size: int = 224,
                  dropout: float = 0.5, seed: int = 0, max_ctas: int = 0, bn_eps: float = 1e-5,
-                 fine_tune_at: Optional[int] = None, augmentation=None):
+                 fine_tune_at: Optional[int] = None, augmentation=None, batchnorm: str = "inference"):
         """``fine_tune_at=k`` (0..19): train ``base.features[k:]`` too, BatchNorm in inference mode (see module doc);
         ``k`` counts feature blocks (0 = stem, 1..17 = inverted-residual blocks, 18 = last 1x1 conv, 19 = head only).
         ``augmentation`` (`models.augment.Augmentation`): random flip / rotation / zoom / translation of the input batch
-        in every training step, on the device; evaluation and inference never apply it."""
+        in every training step, on the device; evaluation and inference never apply it.
+        ``batchnorm="training"``: the BatchNorms of ``base.features[k:]`` use batch statistics in training steps and
+        update their running statistics (momentum 0.1, unbiased variance); ``k = 19`` has none, so it is the
+        ``fine_tune_at=19`` engine."""
         from .augment import check_augmentation
-        from .mobilenet import check_fine_tune_at
+        from .mobilenet import check_batchnorm, check_fine_tune_at
 
         ops.require_native()
         self.augmentation = check_augmentation(augmentation)
@@ -64,8 +77,12 @@ class MobileNetV2Engine:
         if image_size % 32:
             raise ValueError("image_size must be a multiple of 32")
         check_fine_tune_at(fine_tune_at)
+        check_batchnorm(batchnorm, fine_tune_at)
         self.fine_tune_at = fine_tune_at
+        self.batchnorm = batchnorm
         self._k = 19 if fine_tune_at is None else fine_tune_at
+        self._bn_train = batchnorm == "training" and self._k <= 18
+        self.bn_momentum = 0.1
         self.batch, self.num_classes, self.image_size = int(batch), int(num_classes), int(image_size)
         self.dropout, self.seed, self.max_ctas, self.bn_eps = float(dropout), seed, int(max_ctas), bn_eps
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
@@ -89,7 +106,22 @@ class MobileNetV2Engine:
         self.params = torch.zeros(off, device=self.device, dtype=torch.float32)
         self.w16 = torch.zeros(off, device=self.device, dtype=torch.bfloat16)
         self.grads: Optional[torch.Tensor] = None
-        self.running = torch.zeros(8, device=self.device)  # no trainable BatchNorm statistics (frozen base)
+        if self._bn_train:
+            # running statistics of the trainable BatchNorms: one flat buffer, means then variances (as ResNet-50)
+            bns = [(bn, cout) for _, _, bn, _, cout, _, _, _, feat in self._layers if feat >= self._k]
+            tot = sum(c for _, c in bns)
+            self.running = torch.zeros(2 * tot, device=self.device)
+            self.running_mean: Dict[str, torch.Tensor] = {}
+            self.running_var: Dict[str, torch.Tensor] = {}
+            o = 0
+            for bn, c in bns:
+                self.running_mean[bn] = self.running[o:o + c]
+                self.running_var[bn] = self.running[tot + o:tot + o + c]
+                o += c
+            self._tracked: Dict[str, int] = {}   # num_batches_tracked at the last load, + training steps since
+            self._tracked_from = 0
+        else:
+            self.running = torch.zeros(8, device=self.device)  # no trainable BatchNorm statistics (frozen base)
         self.grad_hook: Optional[Callable[[int, int], None]] = None
         self.aux_streams: List[torch.cuda.Stream] = []
         self._step_count = 0
@@ -156,8 +188,11 @@ class MobileNetV2Engine:
 
     def refresh_derived_weights(self) -> None:
         """Trainable layers: folded scale / shift from gamma / beta and the frozen statistics, bf16 dgrad filters
-        scale (.) W of the pointwise layers, and the FC dgrad filter.  (The head GEMM reads the flat bf16 copy.)"""
-        if self._built and self._ft_stats:
+        scale (.) W of the pointwise layers, and the FC dgrad filter.  (The head GEMM reads the flat bf16 copy.)
+        With training-mode BatchNorm: the inference affine from the running statistics, and the plain W^T filters."""
+        if self._built and self._bn_train:
+            self._refresh_bn_train()
+        elif self._built and self._ft_stats:
             self._e.mbv2_ft_refresh(self.params, self._ft_refresh_table)
         if getattr(self, "_fc_dg", None) is not None:
             self._e.weight_prep(self.p("fc.weight"), None, self._fc_wd, 1, self.classes_padded, self.feat_channels)
@@ -182,6 +217,11 @@ class MobileNetV2Engine:
         sd["fc.weight"] = self.p("fc.weight")[:self.num_classes].detach().clone().cpu()
         sd["fc.bias"] = self.p("fc.bias").detach().clone().cpu()
         for kind, conv, bn, cin, cout, *_ in self._trainable_layers():
+            if self._bn_train:
+                sd[bn + ".running_mean"] = self.running_mean[bn].detach().clone().cpu()
+                sd[bn + ".running_var"] = self.running_var[bn].detach().clone().cpu()
+                sd[bn + ".num_batches_tracked"] = torch.tensor(
+                    self._tracked[bn] + self._step_count - self._tracked_from, dtype=torch.int64)
             w = self.p(conv + ".weight").detach().cpu()
             if kind == "stem":   # [27, 32] -> [32, 3, 3, 3]
                 sd[conv + ".weight"] = w.view(3, 3, 3, 32).permute(3, 2, 0, 1).contiguous()
@@ -212,6 +252,12 @@ class MobileNetV2Engine:
             inv, mean = self._ft_stats[bn]
             inv[:cout].copy_(torch.rsqrt(sd[bn + ".running_var"].float() + self.bn_eps))   # the host fold of _affine
             mean[:cout].copy_(sd[bn + ".running_mean"].float())
+            if self._bn_train:
+                self.running_mean[bn].copy_(sd[bn + ".running_mean"].float())
+                self.running_var[bn].copy_(sd[bn + ".running_var"].float())
+                self._tracked[bn] = int(sd.get(bn + ".num_batches_tracked", torch.tensor(0)))
+        if self._bn_train:
+            self._tracked_from = self._step_count
         self._e.cast_bf16(self.params, self.w16)
         if self._built:
             self._load_base_weights()
@@ -290,20 +336,110 @@ class MobileNetV2Engine:
                     lay["res_src"] = block_src
                 lay["op"] = C.ConvForward(x, lay["w"], out, 1, 1, 1, 0, None, None, self.max_ctas,
                                           epilogue=(lay["scale"], lay["shift"], act, res))
+                lay["res"] = res
                 if act == "none":
                     # output of an inverted-residual block (linear bottleneck) = the next block's input
                     block_in, block_src = out, len(self._plan)
+            if train and self._bn_train:
+                self._add_bn_train_buffers(lay, N * ho * ho)
             self._plan.append(lay)
             x, h = out, ho
         self.feat = x   # [N, S/32, S/32, 1280]
         self.pooled = torch.zeros(N, self.feat_channels, **bf)
         self._load_base_weights()
-        if self._ft_stats:
+        if self._bn_train:
+            cmax = max(lay["cout"] for lay in self._plan if lay["train"])
+            self._fold_scratch = torch.zeros(4, cmax, **f32)   # sum, sqsum, mean, invstd bn_finalize also writes
+        elif self._ft_stats:
             self._ft_refresh_table = self._table([self._refresh_row(lay) for lay in self._plan if lay["train"]])
         self._built = True
         self._build_head(training)
         self.refresh_derived_weights()
         return self
+
+    # ------------------------------------------------------------------------------------------------ training-mode BN
+    def _add_bn_train_buffers(self, lay: dict, count: int) -> None:
+        """Conv output c, its statistics sums and the batch affine of a trainable layer (cp-sized, zero padding), and
+        for pointwise layers the GEMM writing c with the kStats = 1 statistics epilogue."""
+        dev, cp = self.device, _cp(lay["cout"])
+        lay["c"] = torch.zeros_like(lay["y"])
+        lay["count"] = count
+        lay["ssum"], lay["ssq"], lay["bmean"], lay["binv"], lay["bscale"], lay["bshift"] = \
+            torch.zeros(6, cp, device=dev).unbind(0)
+        if lay["kind"] == "pw":
+            lay["op_stats"] = C.ConvForward(lay["x"], lay["w"], lay["c"], 1, 1, 1, 0, lay["ssum"], lay["ssq"],
+                                            self.max_ctas)
+
+    def _forward_bn_train(self, lay: dict) -> None:
+        """c = conv(x) + statistics, batch affine + running-statistics update, y = act(affine(c) [+ residual])."""
+        e, kind, cout, bn = self._e, lay["kind"], lay["cout"], lay["bn"]
+        if kind == "stem":
+            e.mbv2_stem_stats(self._stem_input(True), lay["w"], lay["c"], lay["ssum"][:32], lay["ssq"][:32],
+                              1.0 / 127.5, -1.0)
+        elif kind == "dw":
+            e.dwconv3x3_stats(lay["x"], lay["w"], lay["c"], lay["ssum"], lay["ssq"], lay["stride"])
+        else:
+            lay["op_stats"].run()
+        e.bn_finalize(lay["ssum"], lay["ssq"], float(lay["count"]), self.p(bn + ".weight"), self.p(bn + ".bias"),
+                      self.running_mean[bn], self.running_var[bn], self.bn_momentum, self.bn_eps, lay["bmean"][:cout],
+                      lay["binv"][:cout], lay["bscale"][:cout], lay["bshift"][:cout], True)
+        act = lay["act"]
+        e.bn_apply(lay["c"], lay["bscale"], lay["bshift"], lay["res"] if kind == "pw" else None, None, None, lay["y"],
+                   act != "none", None, act == "relu6")
+
+    def _refresh_bn_train(self) -> None:
+        """Inference affine of every trainable layer from its running statistics (bn_finalize in inference mode: the
+        padding of scale / shift stays 1 / 0), and the bf16 W^T dgrad filters of the pointwise layers."""
+        e = self._e
+        s_sum, s_sq, s_mean, s_inv = self._fold_scratch.unbind(0)
+        for lay in self._plan:
+            if lay["train"]:
+                bn, c = lay["bn"], lay["cout"]
+                e.bn_finalize(s_sum, s_sq, 1.0, self.p(bn + ".weight"), self.p(bn + ".bias"), self.running_mean[bn],
+                              self.running_var[bn], self.bn_momentum, self.bn_eps, s_mean, s_inv, lay["scale"][:c],
+                              lay["shift"][:c], False)
+        if getattr(self, "_wd_tiles", 0):
+            e.weight_prep_batched(self.params, self._wd16, self._wd_table, self._wd_tiles)
+
+    def _build_bn_train_backward(self, train: List[int]) -> None:
+        """Scratch of the training-mode BatchNorm backward: dc (one buffer, every layer's dc is consumed before the next
+        layer down writes it), the cp-sized coefficients A / B / C per layer, and the plain W^T filters of the pointwise
+        layers that have a data gradient (one weight_prep_batched table)."""
+        dev = self.device
+        self._dc = torch.zeros(max(self._plan[i]["y"].numel() for i in train), device=dev, dtype=torch.bfloat16)
+        self._ones = torch.ones(max(_cp(self._plan[i]["cout"]) for i in train), device=dev)
+        rows, wd_total, tiles = [], 0, 0
+        for i in train:
+            lay = self._plan[i]
+            cp = _cp(lay["cout"])
+            lay["dc"] = self._dc[:lay["y"].numel()].view(lay["y"].shape)
+            lay["cA"], lay["cB"], lay["cC"] = torch.zeros(3, cp, device=dev).unbind(0)
+            if lay["kind"] == "pw" and i > self._ft_lowest:
+                cin_p = _cp(lay["cin"])
+                rows.append([self.spec[lay["conv"] + ".weight"].offset, wd_total, 1, cp, cin_p, tiles])
+                lay["wd_range"] = (wd_total, cp * cin_p)
+                wd_total += cp * cin_p
+                tiles += (cp // 64) * (cin_p // 32)
+        self._wd16 = torch.zeros(max(wd_total, 8), device=dev, dtype=torch.bfloat16)
+        for i in train:
+            lay = self._plan[i]
+            if "wd_range" in lay:
+                o, n = lay["wd_range"]
+                lay["wd"] = self._wd16[o:o + n].view(_cp(lay["cin"]), _cp(lay["cout"]))
+        if rows:
+            self._wd_table, self._wd_tiles = self._table(rows), tiles
+
+    def _backward_bn_train(self, i: int) -> torch.Tensor:
+        """dz with sum(dz), sum(dz*c); dgamma / dbeta and the coefficients; dc = A*dz + B*c + C.  Returns dc."""
+        e, lay = self._e, self._plan[i]
+        bn, c = lay["bn"], lay["cout"]
+        g = lay["g"]
+        e.relu6_mask_reduce(g, lay["g2"], lay["y"], g, lay["sum"], lay["act"] == "relu6", lay["c"], lay["sumc"])
+        e.bn_bwd_coeffs(lay["sum"][:c], lay["sumc"][:c], self.p(bn + ".weight"), lay["bmean"][:c], lay["binv"][:c],
+                        float(lay["count"]), self.g(bn + ".weight"), self.g(bn + ".bias"), lay["cA"][:c],
+                        lay["cB"][:c], lay["cC"][:c])
+        e.bn_bwd_apply(g, lay["c"], None, None, lay["cA"], lay["cB"], lay["cC"], lay["dc"])
+        return lay["dc"]
 
     # ------------------------------------------------------------------------------------------------ fine-tuning tables
     def _table(self, rows: List[List[int]]) -> torch.Tensor:
@@ -343,15 +479,20 @@ class MobileNetV2Engine:
                                   self.dpooled.view(N, 1, 1, F), 1, 1, 1, 0, mc, wbuf=self._fc_wd)
         train = [i for i, lay in enumerate(self._plan) if lay["train"]]
         self._ft_lowest = train[0]
-        self._ft_sums = torch.zeros(sum(_cp(self._plan[i]["cout"]) for i in train), device=self.device)
+        total = sum(_cp(self._plan[i]["cout"]) for i in train)
+        self._ft_sums = torch.zeros(total * (2 if self._bn_train else 1), device=self.device)
         off = 0
         for i in train:
             lay = self._plan[i]
             cp = _cp(lay["cout"])
             lay["sum"] = self._ft_sums[off:off + cp]
+            if self._bn_train:
+                lay["sumc"] = self._ft_sums[total + off:total + off + cp]
             off += cp
             lay["g"] = torch.zeros_like(lay["y"])   # gradient at the output; turned into dz in place
             lay["g2"] = None
+        if self._bn_train:
+            self._build_bn_train_backward(train)
         for i in train:
             lay = self._plan[i]
             if "res_src" in lay and self._plan[lay["res_src"]]["train"]:
@@ -361,12 +502,14 @@ class MobileNetV2Engine:
                 # the wgrad GEMM takes Cout == 64 or a multiple of 128: 128*a + 64 output channels run as two GEMMs
                 G, cp = self.g(lay["conv"] + ".weight"), _cp(lay["cout"])
                 cuts = [0, cp] if cp == 64 or cp % 128 == 0 else [0, cp - 64, cp]
-                lay["wg"] = [C.ConvWgrad(lay["g"][..., a:b], lay["x"], G[a:b], 1, 1, 1, 0, 0, mc, 0)
+                src = lay["dc"] if self._bn_train else lay["g"]   # training-mode BN: the gradient of c
+                lay["wg"] = [C.ConvWgrad(src[..., a:b], lay["x"], G[a:b], 1, 1, 1, 0, 0, mc, 0)
                              for a, b in zip(cuts, cuts[1:])]
                 if i > self._ft_lowest:
-                    lay["dg"] = C.ConvDgrad(lay["g"], w.view(1, *w.shape), self._plan[i - 1]["g"], 1, 1, 1, 0, mc,
+                    lay["dg"] = C.ConvDgrad(src, w.view(1, *w.shape), self._plan[i - 1]["g"], 1, 1, 1, 0, mc,
                                             wbuf=lay["wd"])
-        self._ft_finalize_table = self._table([self._finalize_row(self._plan[i]) for i in train])
+        if not self._bn_train:
+            self._ft_finalize_table = self._table([self._finalize_row(self._plan[i]) for i in train])
 
     def _build_head(self, training: bool) -> None:
         N, ncp, mc = self.batch, self.classes_padded, self.max_ctas
@@ -392,7 +535,9 @@ class MobileNetV2Engine:
         if training and self._augmenter is not None:
             self._augmenter.run()
         for lay in self._plan:
-            if lay["kind"] == "stem":
+            if training and lay["train"] and self._bn_train:
+                self._forward_bn_train(lay)
+            elif lay["kind"] == "stem":
                 e.mbv2_stem(self._stem_input(training), lay["w"], lay["scale"], lay["shift"], lay["y"], 1.0 / 127.5, -1.0)
             elif lay["kind"] == "dw":
                 e.dwconv3x3(lay["x"], lay["w"], lay["scale"], lay["shift"], lay["y"], lay["stride"])
@@ -425,7 +570,10 @@ class MobileNetV2Engine:
         for i in range(len(self._plan) - 1, self._ft_lowest - 1, -1):
             lay = self._plan[i]
             g, kind = lay["g"], lay["kind"]
-            e.relu6_mask_reduce(g, lay["g2"], lay["y"], g, lay["sum"], lay["act"] == "relu6")
+            if self._bn_train:
+                g = self._backward_bn_train(i)   # dc: the gradient of the conv output
+            else:
+                e.relu6_mask_reduce(g, lay["g2"], lay["y"], g, lay["sum"], lay["act"] == "relu6")
             G = self.g(lay["conv"] + ".weight")
             if kind == "pw":
                 for op in lay["wg"]:
@@ -438,8 +586,10 @@ class MobileNetV2Engine:
                 if kind == "pw":
                     lay["dg"].run()
                 else:
-                    e.dw_dgrad(g, lay["w"], lay["scale"], self._plan[i - 1]["g"], lay["stride"])
-        e.mbv2_ft_finalize(self.params, self.w16, self.grads, self._ft_finalize_table)
+                    scale = self._ones[:_cp(lay["cout"])] if self._bn_train else lay["scale"]
+                    e.dw_dgrad(g, lay["w"], scale, self._plan[i - 1]["g"], lay["stride"])
+        if not self._bn_train:   # training-mode BN: the weight gradients of dc are final, dgamma / dbeta written
+            e.mbv2_ft_finalize(self.params, self.w16, self.grads, self._ft_finalize_table)
 
     def _stem_input(self, training: bool) -> torch.Tensor:
         """uint8 batch the stem reads: the augmented copy in training steps, x_u8 otherwise."""

@@ -21,12 +21,13 @@ def _describe(model) -> dict:
                 "seed": model.seed}   # the seed keys the augmentation draws: a reloaded engine continues the sequence
         if desc["arch"] == "mobilenetv2":
             desc["fine_tune_at"] = model.fine_tune_at
+            desc["batchnorm"] = model.batchnorm
         return desc
     from ..models.mobilenet import FrozenBaseClassifier
 
     if isinstance(model, FrozenBaseClassifier):
         return {"arch": "mobilenetv2", "num_classes": model.fc.out_features, "dropout": model.dropout.p,
-                "freeze_base": model.freeze_base, "fine_tune_at": model.fine_tune_at,
+                "freeze_base": model.freeze_base, "fine_tune_at": model.fine_tune_at, "batchnorm": model.batchnorm,
                 "augmentation": _augmentation(model), "augmentation_seed": model.augmentation_seed}
     return {"arch": "pickle"}
 
@@ -84,11 +85,13 @@ def load_model(model_uri: str, batch_size: Optional[int] = None, device=None):
     elif desc.get("engine") and torch.cuda.is_available():  # saved from the native MobileNetV2 engine
         model = build_model(desc["image_size"], desc["image_size"], 3, desc["num_classes"], desc["dropout"],
                             arch="mobilenetv2", batch_size=batch_size or desc["batch"], device=device,
-                            fine_tune_at=desc.get("fine_tune_at"), augmentation=aug, seed=desc.get("seed", 0))
+                            fine_tune_at=desc.get("fine_tune_at"), augmentation=aug, seed=desc.get("seed", 0),
+                            batchnorm=desc.get("batchnorm", "inference"))
         model.load_state_dict(sd)
     else:
         model = build_model(num_classes=desc["num_classes"], dropout=desc["dropout"], arch="mobilenetv2_torch",
                             freeze_base=desc.get("freeze_base", True), fine_tune_at=desc.get("fine_tune_at"),
-                            augmentation=aug, seed=desc.get("augmentation_seed", 0))
+                            augmentation=aug, seed=desc.get("augmentation_seed", 0),
+                            batchnorm=desc.get("batchnorm", "inference"))
         model.load_state_dict(sd)
     return Trainer(model, device=device)
