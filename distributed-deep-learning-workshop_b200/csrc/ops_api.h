@@ -83,13 +83,17 @@ void weight_prep_batched(const float* params, void* wd, const int64_t* table, in
 
 // Fused flat-buffer optimizers.  `hyper` is a DEVICE array (so LR schedules do not invalidate CUDA graphs):
 //   [0] lr  [1] momentum/beta1  [2] beta2/rho  [3] eps  [4] weight_decay  [5] grad_scale  [6] bias_corr1  [7] bias_corr2
-//   [8] clip threshold  [9] the host's grad_scale  [10..15] unused
-// The update kernels read slots 0-7 only (their bindings accept >= kHyperLen); the clip and LAMB passes need all
+//   [8] clip threshold  [9] the host's grad_scale
+//   [10] EMA decay d  [11] 1 - d  [12] EMA overwrite flag (nonzero: p = ema after the average)  [13..15] unused
+// The update kernels read slots 0-7 only (their bindings accept >= kHyperLen); the clip, LAMB and EMA passes need all
 // kHyperSlots.  The global-norm clip writes [5] = [9] * factor, so repeating a step never compounds the factor.
 constexpr int kHyperLen = 8;
 constexpr int kHyperSlots = 16;
 constexpr int kHypClip = 8;
 constexpr int kHypGradScale = 9;
+constexpr int kHypEmaDecay = 10;
+constexpr int kHypEmaRest = 11;
+constexpr int kHypEmaOverwrite = 12;
 void sgd_step(float* p, const float* g, float* mom, void* p16, int64_t n, const float* hyper, bool nesterov,
               cudaStream_t s);
 void adam_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper, cudaStream_t s);
@@ -120,6 +124,11 @@ void lamb_moments(const float* p, const float* g, float* m, float* v, int64_t n,
                   int64_t nchunks, float* partial, const float* hyper, cudaStream_t s);
 void lamb_apply(float* p, const float* m, const float* v, void* p16, int64_t n, const int64_t* chunks,
                 int64_t nchunks, const float* phi, int nseg, const float* hyper, cudaStream_t s);
+// Gradient accumulation (Keras gradient_accumulation_steps): combine = false: accum += g; combine = true:
+// g = (accum + g) / steps, accum = 0.
+void grad_accumulate(float* g, float* accum, int64_t n, int steps, bool combine, cudaStream_t s);
+// Weight EMA after an update, from hyper slots kHypEmaDecay..kHypEmaOverwrite; p16 may be nullptr.
+void ema_update(float* p, float* ema, void* p16, int64_t n, const float* hyper, cudaStream_t s);
 void cast_f32_to_bf16(const float* x, void* out, int64_t n, cudaStream_t s);
 
 // MobileNetV2 fine-tuning backward (csrc/mobilenet_bwd.cu).  relu6_mask_reduce: with c (training-mode BatchNorm, the

@@ -597,6 +597,46 @@ void lamb_apply(Tensor p, Tensor m, Tensor v, OptT p16, Tensor chunks, Tensor ph
                    phi.data_ptr<float>(), (int)phi.numel(), hyper.data_ptr<float>(), cur());
   after();
 }
+// ---- gradient accumulation and weight EMA: flat fp32 buffers of one size on one device, none overlapping another
+static void disjoint(std::initializer_list<std::pair<const Tensor*, const char*>> ts) {
+  for (auto a = ts.begin(); a != ts.end(); ++a)
+    for (auto b = a + 1; b != ts.end(); ++b) {
+      const auto lo_a = reinterpret_cast<uintptr_t>(a->first->data_ptr()), lo_b = reinterpret_cast<uintptr_t>(b->first->data_ptr());
+      const auto hi_a = lo_a + a->first->nbytes(), hi_b = lo_b + b->first->nbytes();
+      TORCH_CHECK(hi_a <= lo_b || hi_b <= lo_a, a->second, " and ", b->second, " must not overlap");
+    }
+}
+void grad_accumulate(Tensor g, Tensor accum, int64_t steps, int64_t mode) {
+  TORCH_CHECK(mode == 0 || mode == 1, "grad_accumulate: mode 0 (accum += g) or 1 (g = (accum + g) / steps, accum = 0)");
+  TORCH_CHECK(steps >= 1 && steps < (int64_t(1) << 24), "grad_accumulate: steps must be in [1, 2^24)");
+  chk(g, at::kFloat, "g");
+  TORCH_CHECK(g.numel() % 4 == 0, "g: element count must be a multiple of 4");
+  aligned(g, 16, "g");
+  vec(accum, at::kFloat, g.numel(), "accum");
+  TORCH_CHECK(accum.device() == g.device(), "accum must be on the device of g");
+  disjoint({{&g, "g"}, {&accum, "accum"}});
+  b200::grad_accumulate(g.data_ptr<float>(), accum.data_ptr<float>(), g.numel(), (int)steps, mode == 1, cur());
+  after();
+}
+void ema_update(Tensor p, Tensor ema, OptT p16, Tensor hyper) {
+  chk(p, at::kFloat, "p");
+  TORCH_CHECK(p.numel() % 4 == 0, "p: element count must be a multiple of 4");
+  aligned(p, 16, "p");
+  vec(ema, at::kFloat, p.numel(), "ema");
+  vec(hyper, at::kFloat, hyper.numel(), "hyper", 4);
+  TORCH_CHECK(hyper.numel() >= b200::kHyperSlots, "hyper must hold 16 values for the EMA pass");
+  TORCH_CHECK(ema.device() == p.device() && hyper.device() == p.device(), "ema and hyper must be on the device of p");
+  if (p16.has_value()) {
+    vec(*p16, at::kBFloat16, p.numel(), "p16", 8);
+    TORCH_CHECK(p16->device() == p.device(), "p16 must be on the device of p");
+    disjoint({{&p, "p"}, {&ema, "ema"}, {&*p16, "p16"}, {&hyper, "hyper"}});
+  } else {
+    disjoint({{&p, "p"}, {&ema, "ema"}, {&hyper, "hyper"}});
+  }
+  b200::ema_update(p.data_ptr<float>(), ema.data_ptr<float>(), p16.has_value() ? p16->data_ptr() : nullptr, p.numel(),
+                   hyper.data_ptr<float>(), cur());
+  after();
+}
 void cast_bf16(Tensor x, Tensor out) {
   chk(x, at::kFloat, "x");
   TORCH_CHECK(x.numel() % 4 == 0, "x: element count must be a multiple of 4");
@@ -786,6 +826,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("clip_apply", &clip_apply);
   m.def("lamb_moments", &lamb_moments);
   m.def("lamb_apply", &lamb_apply);
+  m.def("grad_accumulate", &grad_accumulate);
+  m.def("ema_update", &ema_update);
   m.def("cast_bf16", &cast_bf16);
   m.def("launch_count", [] { return g_launches; });
   m.def("reset_launch_count", [] { g_launches = 0; });

@@ -405,6 +405,49 @@ __global__ void __launch_bounds__(kChunkThreads) lamb_apply_kernel(float* __rest
   }
 }
 
+// ------------------------------------------------------------------------------------ accumulation and weight EMA
+// IEEE intrinsics throughout (the build uses --use_fast_math): both kernels equal the torch path bit for bit.
+// ACCUMULATE (mode 0): accum += g.  COMBINE (mode 1): g = (accum + g) / n, accum = 0.
+template <bool COMBINE>
+__global__ void grad_accumulate_kernel(float* __restrict__ g, float* __restrict__ accum, int64_t n4, float n) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 gr = reinterpret_cast<float4*>(g)[i];
+    float4 a = reinterpret_cast<float4*>(accum)[i];
+    float* gf = &gr.x; float* af = &a.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if constexpr (COMBINE) {
+        gf[k] = __fdiv_rn(__fadd_rn(af[k], gf[k]), n);
+        af[k] = 0.f;
+      } else {
+        af[k] = __fadd_rn(af[k], gf[k]);
+      }
+    }
+    if (COMBINE) reinterpret_cast<float4*>(g)[i] = gr;
+    reinterpret_cast<float4*>(accum)[i] = a;
+  }
+}
+
+// ema = d * ema + (1 - d) * p with d = hyper[kHypEmaDecay], 1 - d = hyper[kHypEmaRest]; when hyper[kHypEmaOverwrite]
+// is set, p = ema and the bf16 copy is rewritten in the same pass.
+__global__ void ema_update_kernel(float* __restrict__ p, float* __restrict__ ema, __nv_bfloat16* __restrict__ p16,
+                                  int64_t n4, const float* __restrict__ hyper) {
+  const float d = hyper[kHypEmaDecay], d1 = hyper[kHypEmaRest];
+  const bool overwrite = hyper[kHypEmaOverwrite] != 0.f;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+    const float4 w = reinterpret_cast<const float4*>(p)[i];
+    float4 e = reinterpret_cast<float4*>(ema)[i];
+    const float* wf = &w.x; float* ef = &e.x;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) ef[k] = __fadd_rn(__fmul_rn(d, ef[k]), __fmul_rn(d1, wf[k]));
+    reinterpret_cast<float4*>(ema)[i] = e;
+    if (overwrite) {
+      reinterpret_cast<float4*>(p)[i] = e;
+      if (p16 != nullptr) store_bf16x4(p16, i * 4, e);
+    }
+  }
+}
+
 __global__ void cast_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, int64_t n4) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x)
     store_bf16x4(out, i * 4, reinterpret_cast<const float4*>(x)[i]);
@@ -484,6 +527,17 @@ void adadelta_step(float* p, const float* g, float* sq, float* acc, void* p16, i
                    cudaStream_t s) {
   const int64_t n4 = n / 4;
   adadelta_kernel<<<blocks_for(n4), 256, 0, s>>>(p, g, sq, acc, (__nv_bfloat16*)p16, n4, hyper);
+}
+void grad_accumulate(float* g, float* accum, int64_t n, int steps, bool combine, cudaStream_t s) {
+  const int64_t n4 = n / 4;
+  if (combine)
+    grad_accumulate_kernel<true><<<blocks_for(n4), 256, 0, s>>>(g, accum, n4, (float)steps);
+  else
+    grad_accumulate_kernel<false><<<blocks_for(n4), 256, 0, s>>>(g, accum, n4, (float)steps);
+}
+void ema_update(float* p, float* ema, void* p16, int64_t n, const float* hyper, cudaStream_t s) {
+  const int64_t n4 = n / 4;
+  ema_update_kernel<<<blocks_for(n4), 256, 0, s>>>(p, ema, (__nv_bfloat16*)p16, n4, hyper);
 }
 void cast_f32_to_bf16(const float* x, void* out, int64_t n, cudaStream_t s) {
   cast_kernel<<<blocks_for(n / 4), 256, 0, s>>>(x, (__nv_bfloat16*)out, n / 4);

@@ -878,6 +878,10 @@ class EngineTrainStep:
         step.load(x_u8, labels)   # H2D / D2D into the static input buffers (outside the graph)
         step.run()                # graph replay (or eager launches when use_graph=False)
         loss, acc = step.result() # D2H of the two fp32 statistics
+
+    With ``gradient_accumulation_steps`` = n on the optimizer, a second graph is captured: the same launches with the
+    clip, update and EMA passes replaced by one accumulation pass.  `run` replays the update graph on every n-th step
+    and the accumulation graph otherwise; BatchNorm statistics, dropout and augmentation advance on every step.
     """
 
     def __init__(self, engine: ResNet50Engine, optimizer, use_graph: bool = True, warmup_steps: int = 2):
@@ -890,7 +894,8 @@ class EngineTrainStep:
         if self.timeline is not None:
             use_graph = False  # CUDA-event timing cannot be captured into a graph
         self.use_graph = use_graph
-        self.graph: Optional[torch.cuda.CUDAGraph] = None
+        self.graph: Optional[torch.cuda.CUDAGraph] = None          # the update step
+        self.accum_graph: Optional[torch.cuda.CUDAGraph] = None    # the accumulation-only step (n > 1)
         self._dist = hasattr(optimizer, "on_grads_ready")
         if self._dist:
             optimizer.timeline = self.timeline
@@ -916,23 +921,23 @@ class EngineTrainStep:
         self.steps = 0
         self._captured = False
 
-    # one full step as a launch sequence on the current stream
-    def _launch(self) -> None:
+    # one full step as a launch sequence on the current stream; update=False: the accumulation-only variant
+    def _launch(self, update: bool = True) -> None:
         e, opt, tl = self.engine, self.optimizer, self.timeline
         if self._dist:
             opt.start_backward()
         if tl is None:
             e.forward(training=True)
             e.backward()
-            opt.step()  # distributed: waits for the comm stream first
-            e.refresh_derived_weights()
+            opt.step(update)  # distributed: waits for the comm stream first
+            e.refresh_derived_weights()   # also after accumulation: training-mode BatchNorm statistics moved
             return
         with tl.device_span("forward", "step"):
             e.forward(training=True)
         with tl.device_span("backward", "step"):
             e.backward()
         with tl.device_span("allreduce_wait+optimizer", "step"):
-            opt.step()
+            opt.step(update)
         with tl.device_span("weight_relayout", "step"):
             e.refresh_derived_weights()
 
@@ -946,18 +951,25 @@ class EngineTrainStep:
         p0 = e.params.clone()
         r0 = e.running.clone()
         st0 = {k: v.clone() for k, v in self._opt_state().items()}
+        variants = (True, False) if self._opt().accumulation_steps > 1 else (True,)
         s = torch.cuda.Stream(device=e.device)
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):
-            for _ in range(self._warmup_steps):
-                self._launch()
+            for update in variants:
+                for _ in range(self._warmup_steps):
+                    self._launch(update)
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         if self.use_graph:
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self._launch()
-            torch.cuda.synchronize()
+            for update in variants:
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    self._launch(update)
+                torch.cuda.synchronize()
+                if update:
+                    self.graph = g
+                else:
+                    self.accum_graph = g
         e.params.copy_(p0)
         e.running.copy_(r0)
         for k, v in self._opt_state().items():
@@ -965,9 +977,11 @@ class EngineTrainStep:
         e.sync_weights()
         torch.cuda.synchronize()
 
+    def _opt(self):
+        return self.optimizer.opt if self._dist else self.optimizer
+
     def _opt_state(self):
-        o = self.optimizer.opt if self._dist else self.optimizer
-        return o.state
+        return self._opt().state
 
     def load(self, x_u8: torch.Tensor, labels: torch.Tensor) -> None:
         self.engine.set_input(x_u8, labels)
@@ -980,11 +994,13 @@ class EngineTrainStep:
         if getattr(self.engine, "augmentation", None) is not None:
             # written to device memory before every replay: the augmentation draws depend on the step, and a graph
             # captures kernel arguments by value (warm-up in capture() never writes the word, so step 1 sees t = 1)
-            self.engine.set_augment_step((self.optimizer.opt if self._dist else self.optimizer).t)
-        if self.graph is not None:
-            self.graph.replay()
+            self.engine.set_augment_step(self._opt().t)
+        update = self.optimizer.is_update_step
+        graph = self.graph if update else self.accum_graph
+        if graph is not None:
+            graph.replay()
         else:
-            self._launch()
+            self._launch(update)
         self.steps += 1
 
     def result_async(self) -> torch.Tensor:

@@ -10,6 +10,13 @@ Every optimizer takes Keras's ``clipnorm`` / ``clipvalue`` / ``global_clipnorm``
 (a "segment" of the flat buffer: the ``segments`` given to `attach`) and are reduced on the device in a fixed order,
 with no atomics and no host sync, so a clipped step is bit-reproducible and stays inside the step's CUDA graph.
 `Lamb` uses the same segmented reduction for its per-tensor trust ratio.
+
+Every optimizer also takes Keras's ``gradient_accumulation_steps`` (n) and ``use_ema`` / ``ema_momentum`` /
+``ema_overwrite_frequency``.  ``t`` counts training steps (micro-batches, Keras's ``iterations``); step t applies an
+update when t % n == 0, and otherwise only adds the gradient to the ``accum`` state buffer.  An update step uses
+(accum + g) / n, then clips, updates and averages the weights into the ``ema`` state buffer.  Bias corrections count
+applied updates, u = t // n, as torch's ``step()`` does (Keras counts micro-steps there).  The EMA advances once per
+update and ``ema_overwrite_frequency`` counts updates (Keras: micro-steps); at n = 1 both equal Keras.
 """
 from __future__ import annotations
 
@@ -17,9 +24,11 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
-# hyper array layout shared with csrc/ops_api.h: slots 0-7 are read by the update kernels, 8-9 by the clip passes
+# hyper array layout shared with csrc/ops_api.h: slots 0-7 are read by the update kernels, 8-9 by the clip passes,
+# 10-12 by the EMA pass (decay d, 1 - d, overwrite flag: nonzero makes the pass write p = ema and the bf16 copy)
 LR, MOM, BETA2, EPS, WD, GSCALE, BC1, BC2 = range(8)
 CLIP, HOST_GSCALE = 8, 9
+EMA_DECAY, EMA_REST, EMA_OVERWRITE = 10, 11, 12
 HYPER_SLOTS = 16
 CHUNK = 8192   # floats per chunk of the segmented reductions (csrc/ops_api.h kChunkMax)
 CLIP_MODES = ("clipnorm", "clipvalue", "global_clipnorm")
@@ -63,7 +72,19 @@ class FlatOptimizer:
     name = "base"
 
     def __init__(self, learning_rate: float = 1e-3, weight_decay: float = 0.0, clipnorm: Optional[float] = None,
-                 clipvalue: Optional[float] = None, global_clipnorm: Optional[float] = None):
+                 clipvalue: Optional[float] = None, global_clipnorm: Optional[float] = None,
+                 gradient_accumulation_steps: Optional[int] = None, use_ema: bool = False, ema_momentum: float = 0.99,
+                 ema_overwrite_frequency: Optional[int] = None):
+        self.gradient_accumulation_steps = self._check_count("gradient_accumulation_steps",
+                                                             gradient_accumulation_steps, 2)
+        self.use_ema = bool(use_ema)
+        self.ema_momentum = ema_momentum
+        self.ema_overwrite_frequency = ema_overwrite_frequency
+        if self.use_ema:   # as Keras: the EMA arguments are only checked (and read) with use_ema
+            self.ema_momentum = float(ema_momentum)
+            if not 0.0 <= self.ema_momentum <= 1.0:
+                raise ValueError(f"ema_momentum must be in [0, 1], got {ema_momentum}")
+            self.ema_overwrite_frequency = self._check_count("ema_overwrite_frequency", ema_overwrite_frequency, 1)
         self.learning_rate = float(learning_rate)
         self.weight_decay = float(weight_decay)
         self.grad_scale = 1.0
@@ -123,6 +144,43 @@ class FlatOptimizer:
         """'clipnorm', 'clipvalue', 'global_clipnorm' or None."""
         return next((k for k in CLIP_MODES if self._clip[k] is not None), None)
 
+    # -- gradient accumulation and weight EMA (Keras semantics; see the module docstring for the differences)
+    @staticmethod
+    def _check_count(name: str, v: Optional[int], least: int) -> Optional[int]:
+        if v is None:
+            return None
+        if isinstance(v, bool) or not isinstance(v, int) or v < least:
+            raise ValueError(f"{name} must be an integer >= {least} or None, got {v!r}")
+        return v
+
+    @property
+    def accumulation_steps(self) -> int:
+        """n: micro-batches per applied update (1 without gradient accumulation)."""
+        return self.gradient_accumulation_steps or 1
+
+    @property
+    def updates(self) -> int:
+        """u = t // n: updates applied after step t (torch's ``step()`` count; the bias corrections use it)."""
+        return self.t // self.accumulation_steps
+
+    @property
+    def is_update_step(self) -> bool:
+        """Whether step ``t`` (after `begin_step`) applies an update rather than only accumulating."""
+        return self.t % self.accumulation_steps == 0
+
+    def seed_ema(self) -> None:
+        """ema = the current parameters (after loading weights that carry no average)."""
+        if "ema" in self.state:
+            self.state["ema"].copy_(self.params)
+
+    def finalize_variable_values(self) -> None:
+        """Keras's end of ``fit`` with ``use_ema``: the parameters (and the bf16 copy) become the moving average."""
+        if "ema" not in self.state:
+            return
+        self.params.copy_(self.state["ema"])
+        if self.w16 is not None:
+            self.w16.copy_(self.params)
+
     def attach(self, params: torch.Tensor, grads: torch.Tensor, w16: Optional[torch.Tensor] = None,
                segments: Optional[Sequence[Tuple[int, int]]] = None) -> "FlatOptimizer":
         """Bind the flat buffers.  ``segments``: the [lo, hi) range of every parameter tensor (per-tensor clip norms,
@@ -133,6 +191,10 @@ class FlatOptimizer:
         self.segments = normalize_segments(segments, params.numel())
         for k in self._state_names():
             self.state[k] = torch.full_like(params, self._state_init(k))
+        if self.gradient_accumulation_steps is not None:
+            self.state["accum"] = torch.zeros_like(params)
+        if self.use_ema:
+            self.state["ema"] = params.clone()
         self._hyper = torch.zeros(HYPER_SLOTS, device=params.device, dtype=torch.float32)
         if params.is_cuda:
             from .. import ops
@@ -178,6 +240,13 @@ class FlatOptimizer:
         h[BC2] = 1.0
         h[CLIP] = self._clip[mode] if mode is not None else 0.0
         h[HOST_GSCALE] = self.grad_scale
+        if self.use_ema:
+            # for the update of step t (u = t // n): d = 0 on the first update (Keras seeds the average with it)
+            u, f = self.updates, self.ema_overwrite_frequency
+            d = self.ema_momentum if u > 1 else 0.0
+            h[EMA_DECAY] = d
+            h[EMA_REST] = 1.0 - d
+            h[EMA_OVERWRITE] = 1.0 if f is not None and u >= 1 and u % f == 0 else 0.0
 
     def push_hyper(self) -> None:
         """Host -> device copy of the hyper-parameters (outside any CUDA graph)."""
@@ -193,14 +262,50 @@ class FlatOptimizer:
         self.t += 1
         self.push_hyper()
 
-    def step(self) -> None:
-        """Clip the gradient when a clip option is set, then update (all launches capturable in a CUDA graph)."""
-        if self.params.is_cuda:
+    def step(self, update: Optional[bool] = None) -> None:
+        """One training step (all launches capturable in a CUDA graph).  An update step combines the accumulated
+        gradient with this one, clips it when a clip option is set, updates, then advances the weight EMA; any other
+        step only adds the gradient to ``accum``.  ``update``: None decides from ``t`` (`is_update_step`); a captured
+        graph fixes it per variant."""
+        if update is None:
+            update = self.is_update_step
+        n = self.accumulation_steps
+        if n == 1 and not update:
+            raise ValueError("step(update=False) needs gradient_accumulation_steps")
+        cuda = self.params.is_cuda
+        if n > 1:
+            if cuda:
+                self._ext.grad_accumulate(self.grads, self.state["accum"], n, 1 if update else 0)
+            else:
+                self._accumulate_torch(update)
+            if not update:
+                return
+        if cuda:
             self._clip_cuda()
             self._step_cuda()
+            if self.use_ema:
+                self._ext.ema_update(self.params, self.state["ema"], self.w16, self._hyper)
         else:
             self._clip_torch()
             self._step_torch()
+            if self.use_ema:
+                self._ema_torch()
+
+    def _accumulate_torch(self, update: bool) -> None:
+        g, acc = self.grads, self.state["accum"]
+        if update:
+            g.add_(acc).div_(self.accumulation_steps)   # acc + g: IEEE addition commutes, so this is the kernel's sum
+            acc.zero_()
+        else:
+            acc.add_(g)
+
+    def _ema_torch(self) -> None:
+        h, e = self._hyper, self.state["ema"]
+        e.mul_(h[EMA_DECAY]).add_(self.params * h[EMA_REST])
+        if bool(h[EMA_OVERWRITE] != 0):
+            self.params.copy_(e)
+            if self.w16 is not None:
+                self.w16.copy_(self.params)
 
     def _clip_cuda(self) -> None:
         mode = self.clip_mode
@@ -245,7 +350,13 @@ class FlatOptimizer:
         self.t = sd["t"]
         self.learning_rate = sd["lr"]
         for k, v in sd["state"].items():
+            if k in ("accum", "ema") and k not in self.state:
+                continue   # written with accumulation / EMA, resumed without
             self.state[k].copy_(v)
+        if "accum" in self.state and "accum" not in sd["state"]:
+            self.state["accum"].zero_()
+        if "ema" not in sd["state"]:
+            self.seed_ema()
         self.push_hyper()
 
 
@@ -253,8 +364,8 @@ class SGD(FlatOptimizer):
     name = "SGD"
 
     def __init__(self, learning_rate: float = 0.01, momentum: float = 0.0, nesterov: bool = False,
-                 weight_decay: float = 0.0, **clip):
-        super().__init__(learning_rate, weight_decay, **clip)
+                 weight_decay: float = 0.0, **kwargs):
+        super().__init__(learning_rate, weight_decay, **kwargs)
         self.momentum = float(momentum)
         self.nesterov = bool(nesterov)
 
@@ -283,8 +394,8 @@ class Adam(FlatOptimizer):
     name = "Adam"
 
     def __init__(self, learning_rate: float = 1e-3, beta_1: float = 0.9, beta_2: float = 0.999, epsilon: float = 1e-7,
-                 weight_decay: float = 0.0, **clip):
-        super().__init__(learning_rate, weight_decay, **clip)
+                 weight_decay: float = 0.0, **kwargs):
+        super().__init__(learning_rate, weight_decay, **kwargs)
         self.beta_1, self.beta_2, self.epsilon = float(beta_1), float(beta_2), float(epsilon)
 
     def _state_names(self):
@@ -295,7 +406,7 @@ class Adam(FlatOptimizer):
         h[MOM] = self.beta_1
         h[BETA2] = self.beta_2
         h[EPS] = self.epsilon
-        t = max(self.t, 1)
+        t = max(self.updates, 1)
         h[BC1] = 1.0 - self.beta_1 ** t
         h[BC2] = 1.0 - self.beta_2 ** t
 
@@ -318,8 +429,8 @@ class Adadelta(FlatOptimizer):
     name = "Adadelta"
 
     def __init__(self, learning_rate: float = 1e-3, rho: float = 0.95, epsilon: float = 1e-7,
-                 weight_decay: float = 0.0, **clip):
-        super().__init__(learning_rate, weight_decay, **clip)
+                 weight_decay: float = 0.0, **kwargs):
+        super().__init__(learning_rate, weight_decay, **kwargs)
         self.rho, self.epsilon = float(rho), float(epsilon)
 
     def _state_names(self):
@@ -350,8 +461,8 @@ class RMSprop(FlatOptimizer):
     name = "RMSprop"
 
     def __init__(self, learning_rate: float = 1e-3, rho: float = 0.9, momentum: float = 0.0, epsilon: float = 1e-7,
-                 centered: bool = False, weight_decay: float = 0.0, **clip):
-        super().__init__(learning_rate, weight_decay, **clip)
+                 centered: bool = False, weight_decay: float = 0.0, **kwargs):
+        super().__init__(learning_rate, weight_decay, **kwargs)
         self.rho, self.momentum, self.epsilon = float(rho), float(momentum), float(epsilon)
         self.centered = bool(centered)
 
@@ -393,8 +504,8 @@ class Adagrad(FlatOptimizer):
     name = "Adagrad"
 
     def __init__(self, learning_rate: float = 1e-3, initial_accumulator_value: float = 0.1, epsilon: float = 1e-7,
-                 weight_decay: float = 0.0, **clip):
-        super().__init__(learning_rate, weight_decay, **clip)
+                 weight_decay: float = 0.0, **kwargs):
+        super().__init__(learning_rate, weight_decay, **kwargs)
         self.initial_accumulator_value, self.epsilon = float(initial_accumulator_value), float(epsilon)
 
     def _state_names(self):
@@ -425,8 +536,8 @@ class Adamax(FlatOptimizer):
     name = "Adamax"
 
     def __init__(self, learning_rate: float = 1e-3, beta_1: float = 0.9, beta_2: float = 0.999, epsilon: float = 1e-7,
-                 weight_decay: float = 0.0, **clip):
-        super().__init__(learning_rate, weight_decay, **clip)
+                 weight_decay: float = 0.0, **kwargs):
+        super().__init__(learning_rate, weight_decay, **kwargs)
         self.beta_1, self.beta_2, self.epsilon = float(beta_1), float(beta_2), float(epsilon)
 
     def _state_names(self):
@@ -437,7 +548,7 @@ class Adamax(FlatOptimizer):
         h[MOM] = self.beta_1
         h[BETA2] = self.beta_2
         h[EPS] = self.epsilon
-        h[BC1] = 1.0 - self.beta_1 ** max(self.t, 1)
+        h[BC1] = 1.0 - self.beta_1 ** max(self.updates, 1)
 
     def _step_cuda(self):
         self._ext.adamax_step(self.params, self.grads, self.state["m"], self.state["u"], self.w16, self._hyper)
@@ -458,8 +569,8 @@ class AdamW(Adam):
     name = "AdamW"
 
     def __init__(self, learning_rate: float = 1e-3, beta_1: float = 0.9, beta_2: float = 0.999, epsilon: float = 1e-7,
-                 weight_decay: float = 0.004, **clip):
-        super().__init__(learning_rate, beta_1, beta_2, epsilon, weight_decay, **clip)
+                 weight_decay: float = 0.004, **kwargs):
+        super().__init__(learning_rate, beta_1, beta_2, epsilon, weight_decay, **kwargs)
 
     def _step_cuda(self):
         self._ext.adamw_step(self.params, self.grads, self.state["m"], self.state["v"], self.w16, self._hyper)

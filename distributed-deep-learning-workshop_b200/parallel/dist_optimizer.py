@@ -115,10 +115,13 @@ class DistributedOptimizer:
     def allocate_weights(self, params: torch.Tensor, w16: Optional[torch.Tensor]):
         """fused_update only: move the fp32 master (and bf16 copy) into symmetric + multicast memory.  Returns the
         (params, w16) tensors the model must use from now on, or the inputs unchanged when fusion is unavailable."""
-        # the per-bucket kernel sees one bucket at a time, so it cannot apply a clip that needs the whole gradient
+        # the per-bucket kernel sees one bucket at a time, so it cannot apply a clip that needs the whole gradient; it
+        # updates every step and has no accumulation or EMA pass
         ok = (self.fused_update and self.world > 1 and params.is_cuda and self._sym is not None
               and self._sym.has_multicast and getattr(self.opt, "name", "") == "SGD" and not self.opt.nesterov
-              and getattr(self.opt, "clip_mode", None) is None)
+              and getattr(self.opt, "clip_mode", None) is None
+              and getattr(self.opt, "gradient_accumulation_steps", None) is None
+              and not getattr(self.opt, "use_ema", False))
         if not ok:
             self.fused_update = False
             return params, w16
@@ -257,10 +260,16 @@ class DistributedOptimizer:
         if self._comm_stream is not None:
             torch.cuda.current_stream().wait_stream(self._comm_stream)
 
-    def step(self) -> None:
+    @property
+    def is_update_step(self) -> bool:
+        return self.opt.is_update_step
+
+    def step(self, update: Optional[bool] = None) -> None:
+        """Every micro-batch is all-reduced (the sum is linear, so accumulating reduced gradients is exact); ``update``
+        as in `FlatOptimizer.step`."""
         self.finish_backward()
         if not self.fused_update:
-            self.opt.step()  # fused_update: the per-bucket kernels already updated and broadcast the weights
+            self.opt.step(update)  # fused_update: the per-bucket kernels already updated and broadcast the weights
         else:
             self._state_complete = False   # momentum now differs per rank outside the owned slices
 

@@ -304,6 +304,7 @@ class Trainer:
         self.stop_training = False
         is_chief = dist_core.rank() == 0
         it = iter(x)
+        steps_run = 0
         cbs.call("on_train_begin", {})
         for epoch in range(initial_epoch, epochs):
             cbs.call("on_epoch_begin", epoch, {})
@@ -321,6 +322,7 @@ class Trainer:
                     except StopIteration:
                         raise ValueError("fit(): the dataset yields no batches (fewer rows than batch_size?)") from None
                 self.backend.train_batch(xb, yb)
+                steps_run += 1
                 for l, a in self.backend.pop_results(keep=1):  # lag one step: keeps H2D/compute overlapped
                     tot_loss += l
                     tot_acc += a
@@ -347,6 +349,12 @@ class Trainer:
                 print(f"Epoch {epoch + 1}/{epochs} - {dt:.1f}s - {msg} - {logs['images_per_sec']:.0f} img/s", flush=True)
             if self.stop_training:
                 break
+        opt = self._flat_optimizer()
+        if getattr(opt, "use_ema", False) and steps_run > 0:
+            # as Keras's fit: the weights become their moving average before on_train_end, so callbacks that save or
+            # log the model there (autolog, checkpoints) see the weights the trainer keeps
+            opt.finalize_variable_values()
+            self.backend.after_state_change()
         cbs.call("on_train_end", {})
         step = getattr(self.backend, "step", None)
         if step is not None and getattr(step, "timeline", None) is not None:
@@ -442,6 +450,16 @@ class Trainer:
 
     def load_weights(self, path: str) -> None:
         self.backend.load_state_dict(torch.load(path, map_location="cpu"))
+        self._seed_ema()
+
+    def _flat_optimizer(self):
+        return self.optimizer.opt if hasattr(self.optimizer, "opt") else self.optimizer
+
+    def _seed_ema(self) -> None:
+        """Loaded weights without a moving average (``use_ema``) start a new one from themselves."""
+        opt = self._flat_optimizer()
+        if opt is not None and hasattr(opt, "seed_ema"):
+            opt.seed_ema()
 
     def save(self, path: str) -> None:
         """Weights + optimizer state + step counter.  With `DistributedOptimizer(fused_update=True)` the momentum is sharded
@@ -450,7 +468,7 @@ class Trainer:
         if getattr(self.optimizer, "state_is_sharded", False):
             raise RuntimeError("the optimizer state is sharded over ranks (fused_update): call "
                                "optimizer.consolidate_state() on every rank before Trainer.save(), or use save_weights()")
-        opt = self.optimizer.opt if hasattr(self.optimizer, "opt") else self.optimizer
+        opt = self._flat_optimizer()
         torch.save({"weights": self.backend.state_dict(), "optimizer": opt.state_dict() if opt is not None else None,
                     "arch": getattr(self.model, "arch", type(self.model).__name__)}, path)
 
@@ -464,8 +482,9 @@ class Trainer:
         ck = torch.load(path, map_location="cpu")
         weights = ck["weights"] if isinstance(ck, dict) and "weights" in ck else ck
         self.backend.load_state_dict(weights)
+        self._seed_ema()   # replaced below when the checkpoint's optimizer state carries the average
         if load_optimizer and isinstance(ck, dict) and ck.get("optimizer") is not None and self.optimizer is not None:
-            opt = self.optimizer.opt if hasattr(self.optimizer, "opt") else self.optimizer
+            opt = self._flat_optimizer()
             if ck["optimizer"].get("name") != getattr(opt, "name", None):
                 raise ValueError(f"checkpoint holds {ck['optimizer'].get('name')} state, the trainer was compiled with "
                                  f"{getattr(opt, 'name', type(opt).__name__)}")
