@@ -60,7 +60,7 @@ def main() -> int:
     gl = torch.Generator(device=dev).manual_seed(1000 + rank)
     for step in range(4):
         g_local = torch.randn(numel, device=dev, generator=gl) * (1.0 + 0.25 * rank)
-        # ---- reference: library all-reduce, average, plain fp32 update (same formula as csrc/optim.cu sgd_kernel)
+        # ---- reference: library all-reduce, average, plain fp32 update (same formula as SgdRule in csrc/optim_rules.cuh)
         g_avg = g_local.clone()
         dist.all_reduce(g_avg)
         g_avg /= world

@@ -365,25 +365,25 @@ def case_elementwise():
     pm = p.clone()
     for _ in range(3):
         pr_.grad = gr.clone(); opt.step()
-        e.sgd_step(pm, gr, mom, p16, hyper, False)
-    ok &= report("sgd_step", rel_err(pm, pr_.detach()), 1e-5)
-    ok &= report("sgd_step_bf16", rel_err(p16, pm), 1e-2)
+        e.optim_step("sgd", pm, gr, [mom], p16, hyper)
+    ok &= report("optim_step sgd", rel_err(pm, pr_.detach()), 1e-5)
+    ok &= report("optim_step sgd bf16", rel_err(p16, pm), 1e-2)
     pr_ = p.clone().requires_grad_(True)
     opt = torch.optim.Adam([pr_], lr=0.1, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-4)
     pm = p.clone(); m = torch.zeros(n, device=DEV); v = torch.zeros(n, device=DEV)
     for t in range(1, 4):
         pr_.grad = gr.clone(); opt.step()
         hyper[6] = 1 - 0.9 ** t; hyper[7] = 1 - 0.999 ** t
-        e.adam_step(pm, gr, m, v, None, hyper)
-    ok &= report("adam_step", rel_err(pm, pr_.detach()), 1e-3)
+        e.optim_step("adam", pm, gr, [m, v], None, hyper)
+    ok &= report("optim_step adam", rel_err(pm, pr_.detach()), 1e-3)
     pr_ = p.clone().requires_grad_(True)
     opt = torch.optim.Adadelta([pr_], lr=1.0, rho=0.9, eps=1e-6)
     pm = p.clone(); sq = torch.zeros(n, device=DEV); ac = torch.zeros(n, device=DEV)
     h2 = torch.tensor([1.0, 0.0, 0.9, 1e-6, 0.0, 1.0, 1.0, 1.0], device=DEV)
     for t in range(3):
         pr_.grad = gr.clone(); opt.step()
-        e.adadelta_step(pm, gr, sq, ac, None, h2)
-    ok &= report("adadelta_step", rel_err(pm, pr_.detach()), 1e-3)
+        e.optim_step("adadelta", pm, gr, [sq, ac], None, h2)
+    ok &= report("optim_step adadelta", rel_err(pm, pr_.detach()), 1e-3)
     return ok
 
 

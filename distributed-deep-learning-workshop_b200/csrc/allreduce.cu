@@ -14,6 +14,7 @@
 #include <string>
 
 #include "comm_api.h"
+#include "optim_rules.cuh"
 
 namespace b200 {
 
@@ -303,7 +304,7 @@ allreduce_sgd_nvls_kernel(CommCtx g, CommCtx w, int64_t off, int64_t n, float* _
   const int64_t per = (nvec + g.world - 1) / g.world;
   const int64_t v0 = per * g.rank;
   const int64_t v1 = (v0 + per < nvec) ? v0 + per : nvec;
-  const float lr = hyper[0], mu = hyper[1], wd = hyper[4];
+  const SgdRule<false> sgd(hyper, scale);   // the unfused update's rule, on the gradient scaled by `scale`
   block_barrier(g, 0);
   char* gmc = reinterpret_cast<char*>(g.mc_buf) + off * 4;
   char* wloc = reinterpret_cast<char*>(w.peer_bufs[w.rank]) + off * 4;
@@ -316,11 +317,7 @@ allreduce_sgd_nvls_kernel(CommCtx g, CommCtx w, int64_t off, int64_t n, float* _
     float* wf = &wv.x;
     float* mf = &mv.x;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float d = fmaf(wd, wf[k], gr[k] * scale);
-      mf[k] = fmaf(mu, mf[k], d);
-      wf[k] = fmaf(-lr, mf[k], wf[k]);
-    }
+    for (int k = 0; k < 4; ++k) sgd(wf[k], gr[k], &mf[k]);
     *reinterpret_cast<float4*>(mom + off + i * 4) = mv;
     const float o[4] = {wf[0], wf[1], wf[2], wf[3]};
     mm_st_f32(wmc + i * 16, o);

@@ -85,27 +85,24 @@ void weight_prep_batched(const float* params, void* wd, const int64_t* table, in
 //   [0] lr  [1] momentum/beta1  [2] beta2/rho  [3] eps  [4] weight_decay  [5] grad_scale  [6] bias_corr1  [7] bias_corr2
 //   [8] clip threshold  [9] the host's grad_scale
 //   [10] EMA decay d  [11] 1 - d  [12] EMA overwrite flag (nonzero: p = ema after the average)  [13..15] unused
-// The update kernels read slots 0-7 only (their bindings accept >= kHyperLen); the clip, LAMB and EMA passes need all
+// The update kernels read slots 0-7 only (their binding accepts >= kHyperLen); the clip, LAMB and EMA passes need all
 // kHyperSlots.  The global-norm clip writes [5] = [9] * factor, so repeating a step never compounds the factor.
 constexpr int kHyperLen = 8;
 constexpr int kHyperSlots = 16;
-constexpr int kHypClip = 8;
-constexpr int kHypGradScale = 9;
-constexpr int kHypEmaDecay = 10;
-constexpr int kHypEmaRest = 11;
-constexpr int kHypEmaOverwrite = 12;
-void sgd_step(float* p, const float* g, float* mom, void* p16, int64_t n, const float* hyper, bool nesterov,
-              cudaStream_t s);
-void adam_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper, cudaStream_t s);
-void adadelta_step(float* p, const float* g, float* sq, float* acc, void* p16, int64_t n, const float* hyper,
-                   cudaStream_t s);
-void adamw_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper, cudaStream_t s);
-// mom / avg: nullptr without momentum / when not centered
-void rmsprop_step(float* p, const float* g, float* sq, float* mom, float* avg, void* p16, int64_t n,
-                  const float* hyper, cudaStream_t s);
-void adagrad_step(float* p, const float* g, float* acc, void* p16, int64_t n, const float* hyper, cudaStream_t s);
-void adamax_step(float* p, const float* g, float* m, float* u, void* p16, int64_t n, const float* hyper,
-                 cudaStream_t s);
+enum : int {
+  kHypLr, kHypMom, kHypBeta2, kHypEps, kHypWd, kHypGScale, kHypBc1, kHypBc2,
+  kHypClip, kHypHostGScale, kHypEmaDecay, kHypEmaRest, kHypEmaOverwrite
+};
+// Elementwise update rules (csrc/optim_rules.cuh), one per kernel instantiation.
+enum OptimRule : int {
+  kRuleSgd, kRuleSgdNesterov, kRuleAdam, kRuleAdamW, kRuleAdadelta, kRuleRmsprop, kRuleRmspropMomentum,
+  kRuleRmspropCentered, kRuleRmspropCenteredMomentum, kRuleAdagrad, kRuleAdamax, kNumOptimRules
+};
+// number of state buffers the rule reads and writes
+int optim_rule_states(OptimRule rule);
+// state: optim_rule_states(rule) fp32 buffers of n elements, in the rule's order; p16 may be nullptr
+void optim_step(OptimRule rule, float* p, const float* g, float* const* state, void* p16, int64_t n,
+                const float* hyper, cudaStream_t s);
 // Chunk table: int64 [nchunks, kChunkFields] = (lo, hi, segment), lo / hi multiples of 4, hi - lo <= kChunkMax.
 // Segment table: int64 [nseg, 2] = (first chunk, end chunk).  partial: fp32 [nchunks] (x2 for LAMB);
 // sums: fp32 [2, nseg + 1] (per-segment sums of squares, then the total); factor: fp32 [nseg].

@@ -2,7 +2,9 @@
 #include <ATen/cuda/CUDAContext.h>
 #include <torch/extension.h>
 
+#include <algorithm>
 #include <cstdint>
+#include <string>
 #include <vector>
 
 #include "ops_api.h"
@@ -454,61 +456,41 @@ void weight_prep_batched(Tensor params, Tensor wd, Tensor table, int64_t total) 
                             total, cur());
   after();
 }
-// flat fp32 buffers read as float4, the bf16 working copy written 4 values (8 bytes) at a time
-static void optim_operands(const Tensor& p, std::initializer_list<std::pair<const Tensor*, const char*>> state,
-                           const OptT& p16, const Tensor& hyper) {
+// One elementwise optimizer update (csrc/optim_rules.cuh): rule name -> kernel instantiation; `state` holds the rule's
+// state buffers in its order.  Flat fp32 buffers are read as float4, the bf16 working copy written 8 bytes at a time.
+const std::pair<const char*, b200::OptimRule> kOptimRules[] = {
+    {"sgd", b200::kRuleSgd},
+    {"sgd_nesterov", b200::kRuleSgdNesterov},
+    {"adam", b200::kRuleAdam},
+    {"adamw", b200::kRuleAdamW},
+    {"adadelta", b200::kRuleAdadelta},
+    {"rmsprop", b200::kRuleRmsprop},
+    {"rmsprop_momentum", b200::kRuleRmspropMomentum},
+    {"rmsprop_centered", b200::kRuleRmspropCentered},
+    {"rmsprop_centered_momentum", b200::kRuleRmspropCenteredMomentum},
+    {"adagrad", b200::kRuleAdagrad},
+    {"adamax", b200::kRuleAdamax},
+};
+void optim_step(const std::string& rule, Tensor p, Tensor g, std::vector<Tensor> state, OptT p16, Tensor hyper) {
+  const auto* it = std::find_if(std::begin(kOptimRules), std::end(kOptimRules),
+                                [&](const auto& r) { return rule == r.first; });
+  TORCH_CHECK(it != std::end(kOptimRules), "optim_step: unknown rule");
+  TORCH_CHECK((int64_t)state.size() == b200::optim_rule_states(it->second),
+              "optim_step: the state list does not hold the rule's state buffers");
   chk(p, at::kFloat, "p");
   TORCH_CHECK(p.numel() % 4 == 0, "p: element count must be a multiple of 4");
   aligned(p, 16, "p");
-  for (const auto& [t, name] : state) vec(*t, at::kFloat, p.numel(), name);
+  vec(g, at::kFloat, p.numel(), "g");
+  std::vector<float*> sp;
+  for (const Tensor& t : state) {
+    vec(t, at::kFloat, p.numel(), "state");
+    sp.push_back(t.data_ptr<float>());
+  }
   if (p16.has_value()) vec(*p16, at::kBFloat16, p.numel(), "p16", 8);
   vec(hyper, at::kFloat, hyper.numel(), "hyper", 1);
   TORCH_CHECK(hyper.numel() >= b200::kHyperLen, "hyper must hold 8 values");
-}
-
-void sgd_step(Tensor p, Tensor g, Tensor mom, OptT p16, Tensor hyper, bool nesterov) {
-  optim_operands(p, {{&g, "g"}, {&mom, "mom"}}, p16, hyper);
-  b200::sgd_step(p.data_ptr<float>(), g.data_ptr<float>(), mom.data_ptr<float>(),
-                 p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), nesterov, cur());
-  after();
-}
-void adam_step(Tensor p, Tensor g, Tensor m, Tensor v, OptT p16, Tensor hyper) {
-  optim_operands(p, {{&g, "g"}, {&m, "m"}, {&v, "v"}}, p16, hyper);
-  b200::adam_step(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
-                  p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
-  after();
-}
-void adadelta_step(Tensor p, Tensor g, Tensor sq, Tensor acc, OptT p16, Tensor hyper) {
-  optim_operands(p, {{&g, "g"}, {&sq, "sq"}, {&acc, "acc"}}, p16, hyper);
-  b200::adadelta_step(p.data_ptr<float>(), g.data_ptr<float>(), sq.data_ptr<float>(), acc.data_ptr<float>(),
-                      p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
-  after();
-}
-void adamw_step(Tensor p, Tensor g, Tensor m, Tensor v, OptT p16, Tensor hyper) {
-  optim_operands(p, {{&g, "g"}, {&m, "m"}, {&v, "v"}}, p16, hyper);
-  b200::adamw_step(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
+  b200::optim_step(it->second, p.data_ptr<float>(), g.data_ptr<float>(), sp.data(),
                    p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
-  after();
-}
-void rmsprop_step(Tensor p, Tensor g, Tensor sq, OptT mom, OptT avg, OptT p16, Tensor hyper) {
-  optim_operands(p, {{&g, "g"}, {&sq, "sq"}}, p16, hyper);
-  if (mom.has_value()) vec(*mom, at::kFloat, p.numel(), "mom");
-  if (avg.has_value()) vec(*avg, at::kFloat, p.numel(), "avg");
-  b200::rmsprop_step(p.data_ptr<float>(), g.data_ptr<float>(), sq.data_ptr<float>(),
-                     mom.has_value() ? mom->data_ptr<float>() : nullptr, avg.has_value() ? avg->data_ptr<float>() : nullptr,
-                     p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
-  after();
-}
-void adagrad_step(Tensor p, Tensor g, Tensor acc, OptT p16, Tensor hyper) {
-  optim_operands(p, {{&g, "g"}, {&acc, "acc"}}, p16, hyper);
-  b200::adagrad_step(p.data_ptr<float>(), g.data_ptr<float>(), acc.data_ptr<float>(),
-                     p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
-  after();
-}
-void adamax_step(Tensor p, Tensor g, Tensor m, Tensor u, OptT p16, Tensor hyper) {
-  optim_operands(p, {{&g, "g"}, {&m, "m"}, {&u, "u"}}, p16, hyper);
-  b200::adamax_step(p.data_ptr<float>(), g.data_ptr<float>(), m.data_ptr<float>(), u.data_ptr<float>(),
-                    p16.has_value() ? p16->data_ptr() : nullptr, p.numel(), hyper.data_ptr<float>(), cur());
   after();
 }
 
@@ -813,14 +795,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("resize_bilinear_u8", &resize_bilinear_u8, py::arg("x"), py::arg("out"), py::arg("planar") = false);
   m.def("weight_prep", &weight_prep);
   m.def("weight_prep_batched", &weight_prep_batched);
-  m.def("sgd_step", &sgd_step);
-  m.def("adam_step", &adam_step);
-  m.def("adadelta_step", &adadelta_step);
-  m.def("adamw_step", &adamw_step);
-  m.def("rmsprop_step", &rmsprop_step, py::arg("p"), py::arg("g"), py::arg("sq"), py::arg("mom"), py::arg("avg"),
-        py::arg("p16"), py::arg("hyper"));
-  m.def("adagrad_step", &adagrad_step);
-  m.def("adamax_step", &adamax_step);
+  m.def("optim_step", &optim_step, py::arg("rule"), py::arg("p"), py::arg("g"), py::arg("state"), py::arg("p16"),
+        py::arg("hyper"));
   m.def("segment_sumsq", &segment_sumsq);
   m.def("segment_finalize", &segment_finalize);
   m.def("clip_apply", &clip_apply);

@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 
 #include "ops_api.h"
+#include "optim_rules.cuh"
 
 namespace b200 {
 
@@ -17,173 +18,35 @@ __device__ __forceinline__ void store_bf16x4(__nv_bfloat16* p16, int64_t i, floa
   *reinterpret_cast<uint2*>(p16 + i) = u;
 }
 
-template <bool NESTEROV>
-__global__ void sgd_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ mom,
-                           __nv_bfloat16* __restrict__ p16, int64_t n4, const float* __restrict__ hyper) {
-  const float lr = hyper[0], mu = hyper[1], wd = hyper[4], gs = hyper[5];
+// One launch of a rule over the flat buffers: per float4, load p, g and the rule's states in order, apply the rule to
+// each lane, store p, the states, then the optional bf16 copy.
+template <int N>
+struct StatePtrs {
+  float* __restrict__ s[N];
+};
+template <class Rule>
+__global__ void update_kernel(float* __restrict__ p, const float* __restrict__ g, StatePtrs<Rule::kStates> st,
+                              __nv_bfloat16* __restrict__ p16, int64_t n4, const float* __restrict__ hyper) {
+  constexpr int S = Rule::kStates;
+  const Rule rule(hyper);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
     float4 w = reinterpret_cast<float4*>(p)[i];
-    float4 gr = reinterpret_cast<const float4*>(g)[i];
-    float4 m = reinterpret_cast<float4*>(mom)[i];
-    float* wf = &w.x; float* gf = &gr.x; float* mf = &m.x;
+    const float4 gr = reinterpret_cast<const float4*>(g)[i];
+    float4 s[S];
+#pragma unroll
+    for (int j = 0; j < S; ++j) s[j] = reinterpret_cast<float4*>(st.s[j])[i];
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      float d = fmaf(wd, wf[k], gf[k] * gs);
-      mf[k] = fmaf(mu, mf[k], d);
-      const float upd = NESTEROV ? fmaf(mu, mf[k], d) : mf[k];
-      wf[k] = fmaf(-lr, upd, wf[k]);
-    }
-    reinterpret_cast<float4*>(p)[i] = w;
-    reinterpret_cast<float4*>(mom)[i] = m;
-    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
-  }
-}
-
-// DECOUPLED (AdamW): p *= 1 - lr * wd before the Adam step, and the gradient carries no L2 term.
-template <bool DECOUPLED>
-__global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m1,
-                            float* __restrict__ v1, __nv_bfloat16* __restrict__ p16, int64_t n4,
-                            const float* __restrict__ hyper) {
-  const float lr = hyper[0], b1 = hyper[1], b2 = hyper[2], eps = hyper[3], wd = hyper[4], gs = hyper[5];
-  const float bc1 = hyper[6], bc2 = hyper[7];
-  const float step = lr / bc1;
-  const float inv_sqrt_bc2 = rsqrtf(bc2);
-  const float decay = 1.f - lr * wd;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 w = reinterpret_cast<float4*>(p)[i];
-    float4 gr = reinterpret_cast<const float4*>(g)[i];
-    float4 m = reinterpret_cast<float4*>(m1)[i];
-    float4 v = reinterpret_cast<float4*>(v1)[i];
-    float* wf = &w.x; float* gf = &gr.x; float* mf = &m.x; float* vf = &v.x;
+      float sk[S];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      float d;
-      if constexpr (DECOUPLED) {
-        wf[k] *= decay;
-        d = gf[k] * gs;
-      } else {
-        d = fmaf(wd, wf[k], gf[k] * gs);
-      }
-      mf[k] = fmaf(b1, mf[k], (1.f - b1) * d);
-      vf[k] = fmaf(b2, vf[k], (1.f - b2) * d * d);
-      const float denom = sqrtf(vf[k]) * inv_sqrt_bc2 + eps;
-      wf[k] = wf[k] - step * mf[k] / denom;
-    }
-    reinterpret_cast<float4*>(p)[i] = w;
-    reinterpret_cast<float4*>(m1)[i] = m;
-    reinterpret_cast<float4*>(v1)[i] = v;
-    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
-  }
-}
-
-__global__ void adadelta_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq,
-                                float* __restrict__ acc, __nv_bfloat16* __restrict__ p16, int64_t n4,
-                                const float* __restrict__ hyper) {
-  const float lr = hyper[0], rho = hyper[2], eps = hyper[3], wd = hyper[4], gs = hyper[5];
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 w = reinterpret_cast<float4*>(p)[i];
-    float4 gr = reinterpret_cast<const float4*>(g)[i];
-    float4 s = reinterpret_cast<float4*>(sq)[i];
-    float4 a = reinterpret_cast<float4*>(acc)[i];
-    float* wf = &w.x; float* gf = &gr.x; float* sf = &s.x; float* af = &a.x;
+      for (int j = 0; j < S; ++j) sk[j] = (&s[j].x)[k];
+      rule((&w.x)[k], (&gr.x)[k], sk);
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float d = fmaf(wd, wf[k], gf[k] * gs);
-      sf[k] = fmaf(rho, sf[k], (1.f - rho) * d * d);
-      const float delta = sqrtf(af[k] + eps) / sqrtf(sf[k] + eps) * d;
-      af[k] = fmaf(rho, af[k], (1.f - rho) * delta * delta);
-      wf[k] = fmaf(-lr, delta, wf[k]);
+      for (int j = 0; j < S; ++j) (&s[j].x)[k] = sk[j];
     }
     reinterpret_cast<float4*>(p)[i] = w;
-    reinterpret_cast<float4*>(sq)[i] = s;
-    reinterpret_cast<float4*>(acc)[i] = a;
-    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
-  }
-}
-
-// torch.optim.RMSprop: v = rho v + (1 - rho) d^2; CENTERED: a = rho a + (1 - rho) d, denom = sqrt(v - a^2) + eps
-// (v - a^2 >= 0 in exact arithmetic; clamped at 0 so that rounding cannot make it NaN); MOMENTUM: buf = mu buf + d / denom,
-// p -= lr buf; otherwise p -= lr d / denom.
-template <bool CENTERED, bool MOMENTUM>
-__global__ void rmsprop_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq,
-                               float* __restrict__ mom, float* __restrict__ avg, __nv_bfloat16* __restrict__ p16,
-                               int64_t n4, const float* __restrict__ hyper) {
-  const float lr = hyper[0], mu = hyper[1], rho = hyper[2], eps = hyper[3], wd = hyper[4], gs = hyper[5];
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 w = reinterpret_cast<float4*>(p)[i];
-    float4 gr = reinterpret_cast<const float4*>(g)[i];
-    float4 s = reinterpret_cast<float4*>(sq)[i];
-    float4 b = MOMENTUM ? reinterpret_cast<float4*>(mom)[i] : float4{};
-    float4 a = CENTERED ? reinterpret_cast<float4*>(avg)[i] : float4{};
-    float* wf = &w.x; float* gf = &gr.x; float* sf = &s.x; float* bf = &b.x; float* af = &a.x;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float d = fmaf(wd, wf[k], gf[k] * gs);
-      sf[k] = fmaf(rho, sf[k], (1.f - rho) * d * d);
-      float var = sf[k];
-      if constexpr (CENTERED) {
-        af[k] = fmaf(rho, af[k], (1.f - rho) * d);
-        var = fmaxf(fmaf(-af[k], af[k], sf[k]), 0.f);
-      }
-      const float q = d / (sqrtf(var) + eps);
-      if constexpr (MOMENTUM) {
-        bf[k] = fmaf(mu, bf[k], q);
-        wf[k] = fmaf(-lr, bf[k], wf[k]);
-      } else {
-        wf[k] = fmaf(-lr, q, wf[k]);
-      }
-    }
-    reinterpret_cast<float4*>(p)[i] = w;
-    reinterpret_cast<float4*>(sq)[i] = s;
-    if (MOMENTUM) reinterpret_cast<float4*>(mom)[i] = b;
-    if (CENTERED) reinterpret_cast<float4*>(avg)[i] = a;
-    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
-  }
-}
-
-// torch.optim.Adagrad (lr_decay 0): acc += d^2, p -= lr d / (sqrt(acc) + eps).
-__global__ void adagrad_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ acc,
-                               __nv_bfloat16* __restrict__ p16, int64_t n4, const float* __restrict__ hyper) {
-  const float lr = hyper[0], eps = hyper[3], wd = hyper[4], gs = hyper[5];
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 w = reinterpret_cast<float4*>(p)[i];
-    float4 gr = reinterpret_cast<const float4*>(g)[i];
-    float4 a = reinterpret_cast<float4*>(acc)[i];
-    float* wf = &w.x; float* gf = &gr.x; float* af = &a.x;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float d = fmaf(wd, wf[k], gf[k] * gs);
-      af[k] = fmaf(d, d, af[k]);
-      wf[k] = fmaf(-lr, d / (sqrtf(af[k]) + eps), wf[k]);
-    }
-    reinterpret_cast<float4*>(p)[i] = w;
-    reinterpret_cast<float4*>(acc)[i] = a;
-    if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
-  }
-}
-
-// torch.optim.Adamax: m = b1 m + (1 - b1) d, u = max(b2 u, |d| + eps), p -= (lr / bc1) m / u.
-__global__ void adamax_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m1,
-                              float* __restrict__ u1, __nv_bfloat16* __restrict__ p16, int64_t n4,
-                              const float* __restrict__ hyper) {
-  const float lr = hyper[0], b1 = hyper[1], b2 = hyper[2], eps = hyper[3], wd = hyper[4], gs = hyper[5];
-  const float step = lr / hyper[6];
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
-    float4 w = reinterpret_cast<float4*>(p)[i];
-    float4 gr = reinterpret_cast<const float4*>(g)[i];
-    float4 m = reinterpret_cast<float4*>(m1)[i];
-    float4 u = reinterpret_cast<float4*>(u1)[i];
-    float* wf = &w.x; float* gf = &gr.x; float* mf = &m.x; float* uf = &u.x;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float d = fmaf(wd, wf[k], gf[k] * gs);
-      mf[k] = fmaf(b1, mf[k], (1.f - b1) * d);
-      uf[k] = fmaxf(b2 * uf[k], fabsf(d) + eps);
-      wf[k] = wf[k] - step * mf[k] / uf[k];
-    }
-    reinterpret_cast<float4*>(p)[i] = w;
-    reinterpret_cast<float4*>(m1)[i] = m;
-    reinterpret_cast<float4*>(u1)[i] = u;
+    for (int j = 0; j < S; ++j) reinterpret_cast<float4*>(st.s[j])[i] = s[j];
     if (p16 != nullptr) store_bf16x4(p16, i * 4, w);
   }
 }
@@ -227,7 +90,7 @@ __device__ __forceinline__ float block_sum(float x, float* red) {
   return x;   // valid in thread 0
 }
 
-// partial[chunk] = sum over the chunk of (g * hyper[kHypGradScale])^2
+// partial[chunk] = sum over the chunk of (g * hyper[kHypHostGScale])^2
 __global__ void __launch_bounds__(kChunkThreads) segment_sumsq_kernel(const float* __restrict__ g, int64_t n,
                                                                       const int64_t* __restrict__ chunks,
                                                                       float* __restrict__ partial,
@@ -235,7 +98,7 @@ __global__ void __launch_bounds__(kChunkThreads) segment_sumsq_kernel(const floa
   __shared__ float red[kChunkThreads / 32];
   Chunk c;
   const bool ok = load_chunk(chunks, n, c);
-  const float gs = hyper[kHypGradScale];
+  const float gs = hyper[kHypHostGScale];
   float acc = 0.f;
   if (ok) {
     for (int64_t i = c.lo4 + threadIdx.x; i < c.hi4; i += kChunkThreads) {
@@ -254,7 +117,7 @@ __global__ void __launch_bounds__(kChunkThreads) segment_sumsq_kernel(const floa
 // One CTA of 32 warps.  Segment s's partials (chunks segs[s].first .. segs[s].end) are summed by one warp: lane l adds
 // chunks first + l, first + l + 32, ... in order, then a shuffle tree; the global sum is the same warp reduction over
 // the segment sums in segment order.  sums[k * (nseg + 1) + s] (k = 0: partial_a, 1: partial_b), global at index nseg.
-// mode kFinClipGlobal: hyper[GSCALE] = hyper[kHypGradScale] * c / max(norm, c) with c = hyper[kHypClip]
+// mode kFinClipGlobal: hyper[kHypGScale] = hyper[kHypHostGScale] * c / max(norm, c) with c = hyper[kHypClip]
 // mode kFinClipNorm:   factor[s] = c / max(norm_s, c)
 // (the clip factor is exactly 1 when the norm does not exceed c)
 // mode kFinLamb:       factor[s] = norm(p)_s / norm(r)_s, or 1 when either is 0 (partial_a: p^2, partial_b: r^2)
@@ -303,7 +166,7 @@ __global__ void __launch_bounds__(kFinThreads) segment_finalize_kernel(const flo
       const float tot = warp_sum_strided(sums + k * (nseg + 1), 0, nseg);
       if (lane == 0) sums[k * (nseg + 1) + nseg] = tot;
       if (k == 0 && lane == 0 && mode == kFinClipGlobal)
-        hyper[5] = hyper[kHypGradScale] * clip_factor(tot, c);
+        hyper[kHypGScale] = hyper[kHypHostGScale] * clip_factor(tot, c);
     }
   }
 }
@@ -315,7 +178,7 @@ __global__ void __launch_bounds__(kChunkThreads) clip_apply_kernel(float* __rest
                                                                    const float* __restrict__ hyper) {
   Chunk c;
   if (!load_chunk(chunks, n, c, factor != nullptr ? nseg : INT32_MAX)) return;
-  const float gs = hyper[kHypGradScale], lim = hyper[kHypClip];
+  const float gs = hyper[kHypHostGScale], lim = hyper[kHypClip];
   const float f = factor != nullptr ? gs * factor[c.seg] : gs;
   for (int64_t i = c.lo4 + threadIdx.x; i < c.hi4; i += kChunkThreads) {
     float4 v = reinterpret_cast<float4*>(g)[i];
@@ -336,7 +199,8 @@ __device__ __forceinline__ float lamb_dir(float m, float v, float w, float inv_b
 struct LambHyper {
   float b1, b2, eps, wd, gs, inv_bc1, inv_sqrt_bc2;
   __device__ explicit LambHyper(const float* __restrict__ h)
-      : b1(h[1]), b2(h[2]), eps(h[3]), wd(h[4]), gs(h[5]), inv_bc1(1.f / h[6]), inv_sqrt_bc2(rsqrtf(h[7])) {}
+      : b1(h[kHypMom]), b2(h[kHypBeta2]), eps(h[kHypEps]), wd(h[kHypWd]), gs(h[kHypGScale]), inv_bc1(1.f / h[kHypBc1]),
+        inv_sqrt_bc2(rsqrtf(h[kHypBc2])) {}
 };
 
 // pass 1: m, v update; partial[chunk] = sum p^2, partial[nchunks + chunk] = sum r^2
@@ -391,7 +255,7 @@ __global__ void __launch_bounds__(kChunkThreads) lamb_apply_kernel(float* __rest
   Chunk c;
   if (!load_chunk(chunks, n, c, nseg)) return;
   const LambHyper h(hyper);
-  const float step = -hyper[0] * phi[c.seg];
+  const float step = -hyper[kHypLr] * phi[c.seg];
   for (int64_t i = c.lo4 + threadIdx.x; i < c.hi4; i += kChunkThreads) {
     float4 w = reinterpret_cast<float4*>(p)[i];
     const float4 m = reinterpret_cast<const float4*>(m1)[i];
@@ -460,47 +324,39 @@ static inline int blocks_for(int64_t n4) {
   return (int)b;
 }
 
+template <class Rule>
+static void launch_update(float* p, const float* g, float* const* state, void* p16, int64_t n4, const float* hyper,
+                          cudaStream_t s) {
+  StatePtrs<Rule::kStates> st;
+  for (int j = 0; j < Rule::kStates; ++j) st.s[j] = state[j];
+  update_kernel<Rule><<<blocks_for(n4), 256, 0, s>>>(p, g, st, (__nv_bfloat16*)p16, n4, hyper);
+}
+struct RuleEntry {
+  void (*launch)(float*, const float*, float* const*, void*, int64_t, const float*, cudaStream_t);
+  int states;
+};
+template <class Rule>
+constexpr RuleEntry entry() { return {launch_update<Rule>, Rule::kStates}; }
+constexpr RuleEntry kRules[] = {
+    entry<SgdRule<false>>(),            // kRuleSgd
+    entry<SgdRule<true>>(),             // kRuleSgdNesterov
+    entry<AdamRule<false>>(),           // kRuleAdam
+    entry<AdamRule<true>>(),            // kRuleAdamW
+    entry<AdadeltaRule>(),              // kRuleAdadelta
+    entry<RmspropRule<false, false>>(), // kRuleRmsprop
+    entry<RmspropRule<false, true>>(),  // kRuleRmspropMomentum
+    entry<RmspropRule<true, false>>(),  // kRuleRmspropCentered
+    entry<RmspropRule<true, true>>(),   // kRuleRmspropCenteredMomentum
+    entry<AdagradRule>(),               // kRuleAdagrad
+    entry<AdamaxRule>(),                // kRuleAdamax
+};
+static_assert(sizeof(kRules) / sizeof(kRules[0]) == kNumOptimRules, "one entry per OptimRule");
+
+int optim_rule_states(OptimRule rule) { return kRules[rule].states; }
 // n must be a multiple of 4 (flat buffers are padded by the caller).
-void sgd_step(float* p, const float* g, float* mom, void* p16, int64_t n, const float* hyper, bool nesterov,
-              cudaStream_t s) {
-  const int64_t n4 = n / 4;
-  if (nesterov)
-    sgd_kernel<true><<<blocks_for(n4), 256, 0, s>>>(p, g, mom, (__nv_bfloat16*)p16, n4, hyper);
-  else
-    sgd_kernel<false><<<blocks_for(n4), 256, 0, s>>>(p, g, mom, (__nv_bfloat16*)p16, n4, hyper);
-}
-void adam_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper,
-               cudaStream_t s) {
-  const int64_t n4 = n / 4;
-  adam_kernel<false><<<blocks_for(n4), 256, 0, s>>>(p, g, m, v, (__nv_bfloat16*)p16, n4, hyper);
-}
-void adamw_step(float* p, const float* g, float* m, float* v, void* p16, int64_t n, const float* hyper,
-                cudaStream_t s) {
-  const int64_t n4 = n / 4;
-  adam_kernel<true><<<blocks_for(n4), 256, 0, s>>>(p, g, m, v, (__nv_bfloat16*)p16, n4, hyper);
-}
-void rmsprop_step(float* p, const float* g, float* sq, float* mom, float* avg, void* p16, int64_t n,
-                  const float* hyper, cudaStream_t s) {
-  const int64_t n4 = n / 4;
-  auto* b16 = (__nv_bfloat16*)p16;
-  const int nb = blocks_for(n4);
-  if (avg != nullptr && mom != nullptr)
-    rmsprop_kernel<true, true><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
-  else if (avg != nullptr)
-    rmsprop_kernel<true, false><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
-  else if (mom != nullptr)
-    rmsprop_kernel<false, true><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
-  else
-    rmsprop_kernel<false, false><<<nb, 256, 0, s>>>(p, g, sq, mom, avg, b16, n4, hyper);
-}
-void adagrad_step(float* p, const float* g, float* acc, void* p16, int64_t n, const float* hyper, cudaStream_t s) {
-  const int64_t n4 = n / 4;
-  adagrad_kernel<<<blocks_for(n4), 256, 0, s>>>(p, g, acc, (__nv_bfloat16*)p16, n4, hyper);
-}
-void adamax_step(float* p, const float* g, float* m, float* u, void* p16, int64_t n, const float* hyper,
-                 cudaStream_t s) {
-  const int64_t n4 = n / 4;
-  adamax_kernel<<<blocks_for(n4), 256, 0, s>>>(p, g, m, u, (__nv_bfloat16*)p16, n4, hyper);
+void optim_step(OptimRule rule, float* p, const float* g, float* const* state, void* p16, int64_t n,
+                const float* hyper, cudaStream_t s) {
+  kRules[rule].launch(p, g, state, p16, n / 4, hyper, s);
 }
 void segment_sumsq(const float* g, int64_t n, const int64_t* chunks, int64_t nchunks, float* partial,
                    const float* hyper, cudaStream_t s) {
@@ -522,11 +378,6 @@ void lamb_apply(float* p, const float* m, const float* v, void* p16, int64_t n, 
                 int64_t nchunks, const float* phi, int nseg, const float* hyper, cudaStream_t s) {
   lamb_apply_kernel<<<(unsigned)nchunks, kChunkThreads, 0, s>>>(p, m, v, (__nv_bfloat16*)p16, n, chunks, phi, nseg,
                                                                 hyper);
-}
-void adadelta_step(float* p, const float* g, float* sq, float* acc, void* p16, int64_t n, const float* hyper,
-                   cudaStream_t s) {
-  const int64_t n4 = n / 4;
-  adadelta_kernel<<<blocks_for(n4), 256, 0, s>>>(p, g, sq, acc, (__nv_bfloat16*)p16, n4, hyper);
 }
 void grad_accumulate(float* g, float* accum, int64_t n, int steps, bool combine, cudaStream_t s) {
   const int64_t n4 = n / 4;

@@ -49,8 +49,8 @@ LDFLAGS: Dict[str, List[str]] = {
 HEADERS: Dict[str, List[str]] = {
     "_b200_conv": ["ptx.cuh", "conv_igemm.cuh", "conv_params.h", "conv_api.h"],
     "_b200_probe": ["ptx.cuh", "conv_params.h", "conv_api.h"],
-    "_b200_ops": ["ops_api.h", "hash.cuh"],
-    "_b200_comm": ["comm_api.h"],
+    "_b200_ops": ["ops_api.h", "hash.cuh", "optim_rules.cuh"],
+    "_b200_comm": ["comm_api.h", "optim_rules.cuh", "ops_api.h"],
     "_b200_loader": [],
     "_b200_jpeg": [],
 }

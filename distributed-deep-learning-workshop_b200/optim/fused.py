@@ -70,6 +70,8 @@ def chunk_tables(segments: Sequence[Tuple[int, int]]) -> Tuple[torch.Tensor, tor
 
 class FlatOptimizer:
     name = "base"
+    # weight decay scales p inside the update instead of adding wd * p to the gradient (AdamW, Lamb)
+    _decoupled_decay = False
 
     def __init__(self, learning_rate: float = 1e-3, weight_decay: float = 0.0, clipnorm: Optional[float] = None,
                  clipvalue: Optional[float] = None, global_clipnorm: Optional[float] = None,
@@ -222,7 +224,12 @@ class FlatOptimizer:
         self.grads = grads
 
     def _state_names(self):
+        """The state buffers, in the order the update rule reads them."""
         return ()
+
+    def _rule(self) -> str:
+        """The ``optim_step`` update rule (csrc/optim_rules.cuh): the lower-case name unless the class has variants."""
+        return self.name.lower()
 
     def _state_init(self, name: str) -> float:
         return 0.0
@@ -323,6 +330,19 @@ class FlatOptimizer:
             e.segment_finalize(s["partial"][0], s["segs"], s["sums"], s["factor"], self._hyper, FIN_NORM)
             e.clip_apply(self.grads, s["chunks"], s["factor"], self._hyper)
 
+    def _step_cuda(self) -> None:
+        self._ext.optim_step(self._rule(), self.params, self.grads, [self.state[k] for k in self._state_names()],
+                             self.w16, self._hyper)
+
+    def _step_torch(self) -> None:
+        h = self._hyper
+        d = self.grads * h[GSCALE]
+        if not self._decoupled_decay:
+            d = d + h[WD] * self.params
+        self._update_torch(h, d)
+        if self.w16 is not None:
+            self.w16.copy_(self.params)
+
     def _clip_torch(self) -> None:
         mode = self.clip_mode
         if mode is None:
@@ -376,18 +396,14 @@ class SGD(FlatOptimizer):
         super()._fill_hyper(h)
         h[MOM] = self.momentum
 
-    def _step_cuda(self):
-        self._ext.sgd_step(self.params, self.grads, self.state["momentum"], self.w16, self._hyper, self.nesterov)
+    def _rule(self):
+        return "sgd_nesterov" if self.nesterov else "sgd"
 
-    def _step_torch(self):
-        h = self._hyper
-        d = self.grads * h[GSCALE] + h[WD] * self.params
+    def _update_torch(self, h, d):
         m = self.state["momentum"]
         m.mul_(h[MOM]).add_(d)
         upd = d + h[MOM] * m if self.nesterov else m
         self.params.add_(upd * (-h[LR]))
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
 
 
 class Adam(FlatOptimizer):
@@ -410,19 +426,12 @@ class Adam(FlatOptimizer):
         h[BC1] = 1.0 - self.beta_1 ** t
         h[BC2] = 1.0 - self.beta_2 ** t
 
-    def _step_cuda(self):
-        self._ext.adam_step(self.params, self.grads, self.state["m"], self.state["v"], self.w16, self._hyper)
-
-    def _step_torch(self):
-        h = self._hyper
-        d = self.grads * h[GSCALE] + h[WD] * self.params
+    def _update_torch(self, h, d):
         m, v = self.state["m"], self.state["v"]
         m.mul_(h[MOM]).add_(d * (1 - h[MOM]))
         v.mul_(h[BETA2]).add_(d * d * (1 - h[BETA2]))
         denom = (v / h[BC2]).sqrt() + h[EPS]
         self.params.add_(-(h[LR] / h[BC1]) * m / denom)
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
 
 
 class Adadelta(FlatOptimizer):
@@ -441,19 +450,12 @@ class Adadelta(FlatOptimizer):
         h[BETA2] = self.rho
         h[EPS] = self.epsilon
 
-    def _step_cuda(self):
-        self._ext.adadelta_step(self.params, self.grads, self.state["sq"], self.state["acc"], self.w16, self._hyper)
-
-    def _step_torch(self):
-        h = self._hyper
-        d = self.grads * h[GSCALE] + h[WD] * self.params
+    def _update_torch(self, h, d):
         sq, acc = self.state["sq"], self.state["acc"]
         sq.mul_(h[BETA2]).add_(d * d * (1 - h[BETA2]))
         delta = (acc + h[EPS]).sqrt() / (sq + h[EPS]).sqrt() * d
         acc.mul_(h[BETA2]).add_(delta * delta * (1 - h[BETA2]))
         self.params.add_(-h[LR] * delta)
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
 
 
 class RMSprop(FlatOptimizer):
@@ -475,15 +477,11 @@ class RMSprop(FlatOptimizer):
         h[BETA2] = self.rho
         h[EPS] = self.epsilon
 
-    def _step_cuda(self):
-        # the kernel variant follows the state attach() allocated (momentum > 0, centered)
-        st = self.state
-        self._ext.rmsprop_step(self.params, self.grads, st["v"], st.get("momentum"), st.get("avg_grad"), self.w16,
-                               self._hyper)
+    def _rule(self):
+        return "rmsprop" + ("_centered" if self.centered else "") + ("_momentum" if self.momentum > 0 else "")
 
-    def _step_torch(self):
-        h, st = self._hyper, self.state
-        d = self.grads * h[GSCALE] + h[WD] * self.params
+    def _update_torch(self, h, d):
+        st = self.state
         v = st["v"]
         v.mul_(h[BETA2]).add_(d * d * (1 - h[BETA2]))
         var = v
@@ -495,8 +493,6 @@ class RMSprop(FlatOptimizer):
         if "momentum" in st:
             q = st["momentum"].mul_(h[MOM]).add_(q)
         self.params.add_(q * (-h[LR]))
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
 
 
 class Adagrad(FlatOptimizer):
@@ -518,17 +514,10 @@ class Adagrad(FlatOptimizer):
         super()._fill_hyper(h)
         h[EPS] = self.epsilon
 
-    def _step_cuda(self):
-        self._ext.adagrad_step(self.params, self.grads, self.state["acc"], self.w16, self._hyper)
-
-    def _step_torch(self):
-        h = self._hyper
-        d = self.grads * h[GSCALE] + h[WD] * self.params
+    def _update_torch(self, h, d):
         acc = self.state["acc"]
         acc.add_(d * d)
         self.params.add_(-h[LR] * d / (acc.sqrt() + h[EPS]))
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
 
 
 class Adamax(FlatOptimizer):
@@ -550,42 +539,25 @@ class Adamax(FlatOptimizer):
         h[EPS] = self.epsilon
         h[BC1] = 1.0 - self.beta_1 ** max(self.updates, 1)
 
-    def _step_cuda(self):
-        self._ext.adamax_step(self.params, self.grads, self.state["m"], self.state["u"], self.w16, self._hyper)
-
-    def _step_torch(self):
-        h = self._hyper
-        d = self.grads * h[GSCALE] + h[WD] * self.params
+    def _update_torch(self, h, d):
         m, u = self.state["m"], self.state["u"]
         m.mul_(h[MOM]).add_(d * (1 - h[MOM]))
         torch.maximum(u * h[BETA2], d.abs() + h[EPS], out=u)
         self.params.add_(-(h[LR] / h[BC1]) * m / u)
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
 
 
 class AdamW(Adam):
     """`torch.optim.AdamW`: p *= 1 - lr * weight_decay, then this repo's Adam step on the gradient alone."""
     name = "AdamW"
+    _decoupled_decay = True
 
     def __init__(self, learning_rate: float = 1e-3, beta_1: float = 0.9, beta_2: float = 0.999, epsilon: float = 1e-7,
                  weight_decay: float = 0.004, **kwargs):
         super().__init__(learning_rate, beta_1, beta_2, epsilon, weight_decay, **kwargs)
 
-    def _step_cuda(self):
-        self._ext.adamw_step(self.params, self.grads, self.state["m"], self.state["v"], self.w16, self._hyper)
-
-    def _step_torch(self):
-        h = self._hyper
+    def _update_torch(self, h, d):
         self.params.mul_(1 - h[LR] * h[WD])
-        d = self.grads * h[GSCALE]
-        m, v = self.state["m"], self.state["v"]
-        m.mul_(h[MOM]).add_(d * (1 - h[MOM]))
-        v.mul_(h[BETA2]).add_(d * d * (1 - h[BETA2]))
-        denom = (v / h[BC2]).sqrt() + h[EPS]
-        self.params.add_(-(h[LR] / h[BC1]) * m / denom)
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
+        super()._update_torch(h, d)
 
 
 class Lamb(Adam):
@@ -593,6 +565,7 @@ class Lamb(Adam):
     phi = ||p|| / ||r|| (1 when either norm is 0), p -= lr * phi * r.  Three launches: moments and per-chunk partial
     norms, per-segment phi, then the update with the bf16 copy."""
     name = "Lamb"
+    _decoupled_decay = True
 
     def _uses_chunks(self) -> bool:
         return True
@@ -604,9 +577,7 @@ class Lamb(Adam):
         e.segment_finalize(s["partial"], s["segs"], s["sums"], s["factor"], self._hyper, FIN_LAMB)
         e.lamb_apply(self.params, self.state["m"], self.state["v"], self.w16, s["chunks"], s["factor"], self._hyper)
 
-    def _step_torch(self):
-        h = self._hyper
-        d = self.grads * h[GSCALE]
+    def _update_torch(self, h, d):
         m, v = self.state["m"], self.state["v"]
         m.mul_(h[MOM]).add_(d * (1 - h[MOM]))
         v.mul_(h[BETA2]).add_(d * d * (1 - h[BETA2]))
@@ -615,8 +586,6 @@ class Lamb(Adam):
             pn, rn = self.params[lo:hi].norm(), r[lo:hi].norm()
             phi = pn / rn if (pn > 0 and rn > 0) else 1.0
             self.params[lo:hi].add_(r[lo:hi] * (-h[LR] * phi))
-        if self.w16 is not None:
-            self.w16.copy_(self.params)
 
 
 OPTIMIZERS = {"SGD": SGD, "Adam": Adam, "Adadelta": Adadelta, "sgd": SGD, "adam": Adam, "adadelta": Adadelta,

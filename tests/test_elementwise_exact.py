@@ -930,9 +930,10 @@ def fmaf(a, b, c):
 
 
 @pytest.mark.parametrize("nesterov", [False, True])
-def test_sgd_step(nesterov):
-    """sgd_step, 3 steps (lr 2^-4, momentum 0.875, weight decay 2^-8, grad scale 0.5): parameters and momentum equal
-    an fp32 emulation of the kernel's fmaf sequence bit for bit, and the bf16 working copy == bf16_rn(p)."""
+def test_optim_step_sgd(nesterov):
+    """optim_step sgd / sgd_nesterov, 3 steps (lr 2^-4, momentum 0.875, weight decay 2^-8, grad scale 0.5): parameters
+    and momentum equal an fp32 emulation of the kernel's fmaf sequence bit for bit, and the bf16 working copy ==
+    bf16_rn(p)."""
     e = _ops()
     g = gen(5)
     lr, mu, wd, gs = (torch.tensor(v, device=DEV) for v in (2.0 ** -4, 0.875, 2.0 ** -8, 0.5))
@@ -943,12 +944,12 @@ def test_sgd_step(nesterov):
     h = hyper(lr=2.0 ** -4, mu=0.875, wd=2.0 ** -8, gs=0.5)
     for step in range(3):
         gr = torch.randn(OPT_N, device=DEV, generator=g) * 4
-        e.sgd_step(pt, gr, mt, p16.t, h, nesterov)
+        e.optim_step("sgd_nesterov" if nesterov else "sgd", pt, gr, [mt], p16.t, h)
         d = fmaf(wd, p, gr * gs)
         m = fmaf(mu, m, d)
         p = fmaf(-lr, fmaf(mu, m, d) if nesterov else m, p)
         torch.cuda.synchronize()
-        name = f"sgd_step nesterov={nesterov} step {step}"
+        name = f"optim_step sgd nesterov={nesterov} step {step}"
         loc = lambda i: f"[float4 {i // 4}: block {i // 4 // 256 % RED_CAP} thread {i // 4 % 256}]"   # noqa: E731
         check_equal(name + " p", pt, p, loc)
         check_equal(name + " momentum", mt, m, loc)
@@ -956,8 +957,8 @@ def test_sgd_step(nesterov):
         p16.check_guards(name + " p16")
 
 
-def test_adam_adadelta_step():
-    """adam_step and adadelta_step, one step, against float64.  Each computes with fast-math sqrtf (sqrt.approx:
+def test_optim_step_adam_adadelta():
+    """optim_step adam and adadelta, one step, against float64.  Each computes with fast-math sqrtf (sqrt.approx:
     relative error <= 2^-23, PTX ISA), rsqrtf (2 ulp) and division (div.approx: 2 ulp) and about eight fp32 roundings on
     the update's path; the bound allows 2^-19 relative on the update and one rounding of the parameter (first order).
     The bf16 working copy is bf16_rn of the parameter the kernel wrote, exactly."""
@@ -973,14 +974,14 @@ def test_adam_adadelta_step():
         p16 = Guarded((OPT_N,), BF)
         d = wd * p + gr * gs
         if name == "adam":
-            e.adam_step(pt, gr.float(), st1, st2, p16.t, hv.float())
+            e.optim_step("adam", pt, gr.float(), [st1, st2], p16.t, hv.float())
             m = b1 * s1 + (1 - b1) * d
             v = b2 * s2 + (1 - b2) * d * d
             upd = lr / bc1 * m / (torch.sqrt(v) / math.sqrt(bc2) + eps)
             states = ((m, (b1 * s1).abs() + ((1 - b1) * d).abs()), (v, v))
         else:
             hd = hyper(lr=1.0, b2=0.9, eps=1e-6, wd=wd, gs=gs)
-            e.adadelta_step(pt, gr.float(), st1, st2, p16.t, hd)
+            e.optim_step("adadelta", pt, gr.float(), [st1, st2], p16.t, hd)
             rho, ep = float(hd[2]), float(hd[3])
             sq = rho * s1 + (1 - rho) * d * d
             delta = torch.sqrt(s2 + ep) / torch.sqrt(sq + ep) * d
@@ -1119,9 +1120,9 @@ def test_malformed_inputs_raise():
         "gap_fwd: output size": lambda: e.gap_fwd(b(2, 7, 7, C), b(2, C - 8), 0.0, 0),
         "gap_fwd: C % 8": lambda: e.gap_fwd(b(2, 7, 7, 12), b(2, 12), 0.0, 0),
         "gap_bwd: dout size": lambda: e.gap_bwd(b(3, C), b(2, 7, 7, C), 0.0, 0),
-        "sgd_step: misaligned p": lambda: e.sgd_step(f(68)[1:65], f(64), f(64), None, f(8), False),
-        "sgd_step: short p16": lambda: e.sgd_step(f(64), f(64), f(64), b(60), f(8), False),
-        "adadelta_step: short state": lambda: e.adadelta_step(f(64), f(64), f(60), f(64), None, f(8)),
+        "optim_step sgd: misaligned p": lambda: e.optim_step("sgd", f(68)[1:65], f(64), [f(64)], None, f(8)),
+        "optim_step sgd: short p16": lambda: e.optim_step("sgd", f(64), f(64), [f(64)], b(60), f(8)),
+        "optim_step adadelta: short state": lambda: e.optim_step("adadelta", f(64), f(64), [f(60), f(64)], None, f(8)),
         "dwconv3x3: misaligned weights": lambda: e.dwconv3x3(b(1, 8, 8, C), f(9 * C + 4)[1:9 * C + 1], c, c,
                                                              b(1, 8, 8, C), 1, 4),
     }

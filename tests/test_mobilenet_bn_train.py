@@ -462,23 +462,29 @@ def test_frozen_part_and_padding_stay_fixed(opt_name):
 
 def test_graph_matches_eager_and_warmup_leaves_no_trace():
     """capture() + n replays: num_batches_tracked == n (the warm-up steps were undone); the running statistics are as
-    close to n eager steps as two eager runs are to each other (fp32 atomics)."""
+    close to n eager steps as eager runs are to each other (fp32 atomics).  The distance between two runs varies
+    several-fold from pair to pair, and two runs sometimes agree almost exactly, so a single pair is no yardstick: the
+    graph run's mean distance to five eager runs is compared with the mean distance over the ten eager pairs."""
+    import itertools
+
     from b200ddl import optim
 
     k, n = 4, 3
     x, y = _batch(8, 64, seed=5)
+    eager = [f"eager{i}" for i in range(5)]
     runs = {}
-    for name, graph in (("eager", False), ("eager2", False), ("graph", True)):
+    for name in eager + ["graph"]:
         eng = _engine(k)
-        _run_steps(eng, optim.SGD(0.05, momentum=0.9), x, y, n, use_graph=graph)
+        _run_steps(eng, optim.SGD(0.05, momentum=0.9), x, y, n, use_graph=name == "graph")
         runs[name] = eng.state_dict()
     for nm, v in runs["graph"].items():
         if nm.endswith("num_batches_tracked") and int(nm.split(".")[2]) >= k:
             assert int(v) == n, nm
     stats = [nm for nm in runs["graph"] if "running" in nm and int(nm.split(".")[2]) >= k]
+    pairs = list(itertools.combinations(eager, 2))
     for nm in stats:
-        spread = _rel(runs["eager2"][nm], runs["eager"][nm])
-        diff = _rel(runs["graph"][nm], runs["eager"][nm])
+        spread = sum(_rel(runs[b][nm], runs[a][nm]) for a, b in pairs) / len(pairs)
+        diff = sum(_rel(runs["graph"][nm], runs[a][nm]) for a in eager) / len(eager)
         assert diff <= max(4 * spread, 1e-3), f"{nm}: graph vs eager {diff}, eager runs {spread}"
 
 

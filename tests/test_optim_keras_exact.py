@@ -62,7 +62,7 @@ RMS_VARIANTS = [(c, m) for c in (False, True) for m in (False, True)]
 
 
 @pytest.mark.parametrize("centered,momentum", RMS_VARIANTS)
-def test_rmsprop_step(centered, momentum):
+def test_optim_step_rmsprop(centered, momentum):
     e = _ops()
     g = gen(11)
     p, gr = (torch.randn(OPT_N, device=DEV, generator=g).double() for _ in range(2))
@@ -74,7 +74,8 @@ def test_rmsprop_step(centered, momentum):
     P, V = guarded(p.float()), guarded(v0.float())
     A, B = guarded(a0.float()), guarded(b0.float())
     p16 = Guarded((OPT_N,), BF)
-    e.rmsprop_step(P.t, gr.float(), V.t, B.t if momentum else None, A.t if centered else None, p16.t, hv)
+    rule = "rmsprop" + ("_centered" if centered else "") + ("_momentum" if momentum else "")
+    e.optim_step(rule, P.t, gr.float(), [V.t] + [B.t] * momentum + [A.t] * centered, p16.t, hv)
     torch.cuda.synchronize()
     p, v0, a0, b0 = p.float().double(), v0.float().double(), a0.float().double(), b0.float().double()
     gr = gr.float().double()
@@ -106,7 +107,7 @@ def test_rmsprop_step(centered, momentum):
 
 
 @pytest.mark.parametrize("name", ["adagrad", "adamax", "adamw"])
-def test_adagrad_adamax_adamw_step(name):
+def test_optim_step_adagrad_adamax_adamw(name):
     e = _ops()
     g = gen(12)
     p, gr = (torch.randn(OPT_N, device=DEV, generator=g).float().double() for _ in range(2))
@@ -118,14 +119,14 @@ def test_adagrad_adamax_adamw_step(name):
     P, S1, S2 = guarded(p.float()), guarded(s1.float()), guarded(s2.float())
     p16 = Guarded((OPT_N,), BF)
     if name == "adagrad":
-        e.adagrad_step(P.t, gr.float(), S2.t, p16.t, hv)
+        e.optim_step("adagrad", P.t, gr.float(), [S2.t], p16.t, hv)
         d = wd * p + gr * gs
         acc = s2 + d * d
         upd = lr * d / (acc.sqrt() + eps)
         states = [(S2, acc, acc)]
         pn = p - upd
     elif name == "adamax":
-        e.adamax_step(P.t, gr.float(), S1.t, S2.t, p16.t, hv)
+        e.optim_step("adamax", P.t, gr.float(), [S1.t, S2.t], p16.t, hv)
         d = wd * p + gr * gs
         m = b1 * s1 + (1 - b1) * d
         u = torch.maximum(b2 * s2, d.abs() + eps)
@@ -134,7 +135,7 @@ def test_adagrad_adamax_adamw_step(name):
         states = [(S1, m, mt), (S2, u, u)]
         pn = p - lr / bc1 * m / u
     else:
-        e.adamw_step(P.t, gr.float(), S1.t, S2.t, p16.t, hv)
+        e.optim_step("adamw", P.t, gr.float(), [S1.t, S2.t], p16.t, hv)
         d = gr * gs
         m = b1 * s1 + (1 - b1) * d
         v = b2 * s2 + (1 - b2) * d * d
@@ -393,10 +394,12 @@ def test_malformed_inputs_raise_before_any_launch():
     partial = torch.zeros(2, chunks.shape[0], device=DEV)
     sums, factor = torch.zeros(2, 2, device=DEV), torch.zeros(1, device=DEV)
     bad = [
-        lambda: e.adagrad_step(torch.zeros(n + 4, device=DEV)[1:n + 1], g, m, None, h8),          # misaligned
-        lambda: e.adamax_step(p, g, m, torch.zeros(n - 4, device=DEV), None, h8),                 # short state
-        lambda: e.rmsprop_step(p, g, m, torch.zeros(n - 4, device=DEV), None, None, h8),          # short momentum
-        lambda: e.adamw_step(p, g, m, v, None, torch.zeros(4, device=DEV)),                       # short hyper
+        lambda: e.optim_step("adagrad", torch.zeros(n + 4, device=DEV)[1:n + 1], g, [m], None, h8),  # misaligned
+        lambda: e.optim_step("adamax", p, g, [m, torch.zeros(n - 4, device=DEV)], None, h8),         # short state
+        lambda: e.optim_step("rmsprop_momentum", p, g, [m, torch.zeros(n - 4, device=DEV)], None, h8),  # short mom
+        lambda: e.optim_step("adamw", p, g, [m, v], None, torch.zeros(4, device=DEV)),               # short hyper
+        lambda: e.optim_step("nadam", p, g, [m, v], None, h8),                                       # unknown rule
+        lambda: e.optim_step("adam", p, g, [m], None, h8),                                           # state count
         lambda: e.segment_sumsq(g, chunks, partial[0], h8),                                       # hyper < 16
         lambda: e.clip_apply(g, chunks, None, h8),
         lambda: e.lamb_moments(p, g, m, v, chunks, partial, h8),
