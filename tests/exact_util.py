@@ -90,6 +90,17 @@ def check_sum(name, got, ref, ref_abs, depth):
     return "bounded"
 
 
+def bf16_half_ulp(x):
+    """Half a bf16 ulp of |x| (float64 tensor; 0 where x == 0): the largest error of rounding x to bf16 (nearest even)."""
+    _, e = torch.frexp(x.abs())
+    return torch.where(x != 0, torch.ldexp(torch.ones_like(x), e - 9), torch.zeros_like(x))
+
+
+def bf16_bound(ref, err):
+    """Bound on |bf16(a) - ref| for an fp32 value a with |a - ref| <= err: a's own rounding plus err."""
+    return bf16_half_ulp(ref.abs() + err) + err
+
+
 def to_bf16_exact(ref):
     """bf16 of a float64 tensor holding values exact in fp32 (round to nearest even, like __floats2bfloat162_rn)."""
     assert bool((ref.float().double() == ref).all()), "reference is not exact in fp32"
