@@ -94,6 +94,93 @@ void softmax_ce_head(const void* logits16, int ld, const float* bias, const int6
                                                     (__nv_bfloat16*)dlogits16, loss_rows, stats, B, K, grad_scale);
 }
 
+// softmax_ce_head against a soft target, for MixUp / CutMix and label smoothing (eps):
+//   target_k = (1 - eps) (lambda [k = y] + mu [k = y_partner]) + eps / K,   lambda = 1 - mu,  mu = num / den (mix row)
+//   loss     = sum_k target_k (lse - logit_k) = (1 - eps) (lambda (lse - l_y) + mu (lse - l_p)) + eps / K sum_k (lse - l_k)
+//   dlogits  = (p_k - target_k) * grad_scale;   correct: argmax(logits) == argmax of the unsmoothed target
+//   lambda [k = y] + mu [k = y_partner], lowest index on ties (Keras smooths inside the loss; its accuracy metric sees
+//   the mixed labels without smoothing).
+// sum_k (lse - l_k) is accumulated as sum_k (max - l_k) + K (lse - max): every term is >= 0.  mu is a correctly rounded
+// division (__fdiv_rn, also under --use_fast_math).  With mu = 0 and eps = 0 every product by lambda, 1 - eps, mu or
+// eps / K is by 1 or 0, so each output is bit for bit softmax_ce_head's.  That argmax is decided on the integers: y when
+// 2 num < den, y_partner when 2 num > den, the lower of the two on a tie.
+__global__ void softmax_ce_soft_head_kernel(const __nv_bfloat16* __restrict__ logits16, int ld,
+                                            const float* __restrict__ bias, const int64_t* __restrict__ labels,
+                                            const int4* __restrict__ mix, float eps, float* __restrict__ logits32,
+                                            __nv_bfloat16* __restrict__ dlogits16, float* __restrict__ loss_rows,
+                                            float* __restrict__ stats, int B, int K, float grad_scale) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (warp >= B) return;
+  const __nv_bfloat16* row = logits16 + (int64_t)warp * ld;
+  const int label = (int)labels[warp];
+  int plabel = label, target = label;
+  float mu = 0.f;
+  if (mix != nullptr) {
+    const int4 m0 = mix[2 * warp], m1 = mix[2 * warp + 1];
+    plabel = (int)labels[(unsigned)m0.x < (unsigned)B ? m0.x : warp];
+    mu = __fdiv_rn((float)m1.z, (float)m1.w);
+    if (plabel != label) {
+      const int64_t twice = 2 * (int64_t)m1.z;
+      target = twice < m1.w ? label : twice > m1.w ? plabel : min(label, plabel);
+    }
+  }
+  const float lam = 1.f - mu, keep = 1.f - eps, epsk = __fdiv_rn(eps, (float)K);
+  float mx = -3.0e38f;
+  int amax = 0;
+  for (int k = lane; k < K; k += 32) {
+    const float v = __bfloat162float(row[k]) + bias[k];
+    if (logits32 != nullptr) logits32[(int64_t)warp * K + k] = v;
+    if (v > mx) { mx = v; amax = k; }
+  }
+  for (int o = 16; o; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+    const int oa = __shfl_xor_sync(0xffffffffu, amax, o);
+    if (om > mx || (om == mx && oa < amax)) { mx = om; amax = oa; }
+  }
+  float se = 0.f, sd = 0.f;
+  for (int k = lane; k < K; k += 32) {
+    const float v = __bfloat162float(row[k]) + bias[k];
+    se += __expf(v - mx);
+    sd += mx - v;
+  }
+  for (int o = 16; o; o >>= 1) {
+    se += __shfl_xor_sync(0xffffffffu, se, o);
+    sd += __shfl_xor_sync(0xffffffffu, sd, o);
+  }
+  const float lse = mx + __logf(se);   // as softmax_ce_head writes it (the compiler fuses the log's scale and the add)
+  const float inv = 1.f / se;
+  if (dlogits16 != nullptr) {
+    __nv_bfloat16* drow = dlogits16 + (int64_t)warp * ld;
+    for (int k = lane; k < ld; k += 32) {
+      float d = 0.f;
+      if (k < K) {
+        const float pk = __expf(__bfloat162float(row[k]) + bias[k] - mx) * inv;
+        const float tk = keep * ((k == label ? lam : 0.f) + (k == plabel ? mu : 0.f)) + epsk;
+        d = (pk - tk) * grad_scale;
+      }
+      drow[k] = __float2bfloat16(d);
+    }
+  }
+  if (lane == 0) {
+    const float ly = __bfloat162float(row[label]) + bias[label];
+    const float lp = __bfloat162float(row[plabel]) + bias[plabel];
+    const float l = keep * (lam * (lse - ly) + mu * (lse - lp)) + epsk * (sd + (float)K * (lse - mx));
+    if (loss_rows != nullptr) loss_rows[warp] = l;
+    atomicAdd(stats, l);
+    atomicAdd(stats + 1, amax == target ? 1.f : 0.f);
+  }
+}
+void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const int64_t* labels, const int32_t* mix,
+                          float eps, float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K,
+                          float grad_scale, cudaStream_t s) {
+  const int threads = 128;
+  const int blocks = (B * 32 + threads - 1) / threads;
+  softmax_ce_soft_head_kernel<<<blocks, threads, 0, s>>>((const __nv_bfloat16*)logits16, ld, bias, labels,
+                                                         (const int4*)mix, eps, logits32, (__nv_bfloat16*)dlogits16,
+                                                         loss_rows, stats, B, K, grad_scale);
+}
+
 // dbias[k] = sum_b dlogits16[b, k]   (thread per column: coalesced across k for every row)
 __global__ void fc_bias_grad_kernel(const __nv_bfloat16* __restrict__ dl, int ld, float* __restrict__ dbias, int B, int K) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;

@@ -158,5 +158,21 @@ void augment_params(int32_t* params, const int32_t* step, const int32_t* rot_tab
                     int flip_mode, int32_t zq, int32_t txq, int32_t tyq, cudaStream_t s);
 void augment_warp(const uint8_t* x, uint8_t* out, const int32_t* params, int N, int H, int W, bool reflect, int fill,
                   cudaStream_t s);
+// MixUp / CutMix on top of the geometric warp.  mix: int32 [N, 8] per image = partner, MixUp own weight w (0..256),
+// CutMix box x0 y0 x1 y1 (half-open), then the partner's label weight mu = num / den;  lam_table: int32
+// [2^kAugLamBits][2] = Q16 lambda and Q16 sqrt(1 - lambda) at the Beta(alpha, alpha) quantiles (i + 0.5) / 2^kAugLamBits.
+constexpr int kAugMixFields = 8;
+constexpr int kAugLamBits = 12;
+enum AugMix : int { kMixNone = 0, kMixUp = 1, kCutMix = 2 };
+void augment_mix_params(int32_t* params, int32_t* mix, const int32_t* step, const int32_t* rot_table,
+                        const int32_t* lam_table, int N, int H, int W, uint32_t key, int flip_mode, int32_t zq,
+                        int32_t txq, int32_t tyq, int mode, cudaStream_t s);
+void augment_mix_warp(const uint8_t* x, uint8_t* out, const int32_t* params, const int32_t* mix, int N, int H, int W,
+                      int mode, bool reflect, int fill, cudaStream_t s);
+// softmax_ce_head against the soft target (1 - eps) (lambda [k = y_n] + mu [k = y_partner]) + eps / K; mix may be
+// nullptr (mu = 0: label smoothing alone)
+void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const int64_t* labels, const int32_t* mix,
+                          float eps, float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K,
+                          float grad_scale, cudaStream_t s);
 
 }  // namespace b200

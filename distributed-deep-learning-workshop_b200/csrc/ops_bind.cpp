@@ -305,6 +305,52 @@ void softmax_ce_head(Tensor logits16, Tensor bias, Tensor labels, OptT logits32,
                         (float)grad_scale, cur());
   after();
 }
+// softmax_ce_head against the soft target of label smoothing `eps` and, with `mix` (int32 [B, 8] mix rows of
+// augment_mix_params), the partner's label at weight num / den; see csrc/head_stem.cu
+void softmax_ce_soft_head(Tensor logits16, Tensor bias, Tensor labels, OptT mix, double eps, OptT logits32,
+                          OptT dlogits16, OptT loss_rows, Tensor stats, double grad_scale) {
+  chk(logits16, at::kBFloat16, "logits16");
+  chk(bias, at::kFloat, "bias");
+  chk(labels, at::kLong, "labels");
+  chk(stats, at::kFloat, "stats");
+  TORCH_CHECK(logits16.dim() == 2 && logits16.size(0) >= 1 && bias.numel() >= 1 && bias.numel() <= logits16.size(1) &&
+                  labels.numel() == logits16.size(0),
+              "logits16 must be bf16 [B, ld] with ld >= K = bias.numel() and B = labels.numel() >= 1");
+  TORCH_CHECK(stats.numel() >= 2, "stats must hold [sum loss, correct]");
+  TORCH_CHECK(eps >= 0.0 && eps <= 1.0, "label smoothing must be in [0, 1]");
+  const int B = (int)logits16.size(0), ld = (int)logits16.size(1), K = (int)bias.numel();
+  for (const Tensor* t : {&bias, &labels, &stats})
+    TORCH_CHECK(t->device() == logits16.device(), "bias, labels and stats must be on the device of logits16");
+  if (mix.has_value()) {
+    chk(*mix, at::kInt, "mix");
+    TORCH_CHECK(mix->dim() == 2 && mix->size(0) == B && mix->size(1) == b200::kAugMixFields,
+                "mix must be int32 [B, 8] for the batch's B rows");
+    TORCH_CHECK(mix->device() == logits16.device(), "mix must be on the device of logits16");
+    aligned(*mix, 16, "mix");
+  }
+  if (logits32.has_value()) {
+    chk(*logits32, at::kFloat, "logits32");
+    TORCH_CHECK(logits32->numel() == (int64_t)B * K, "logits32 must hold B x K values");
+  }
+  if (dlogits16.has_value()) {
+    chk(*dlogits16, at::kBFloat16, "dlogits16");
+    TORCH_CHECK(dlogits16->numel() == logits16.numel(), "dlogits16 must have the shape of logits16");
+    TORCH_CHECK(dlogits16->data_ptr() != logits16.data_ptr(), "dlogits16 cannot overwrite logits16");
+  }
+  if (loss_rows.has_value()) {
+    chk(*loss_rows, at::kFloat, "loss_rows");
+    TORCH_CHECK(loss_rows->numel() == B, "loss_rows must hold B values");
+  }
+  for (const OptT* t : {&logits32, &dlogits16, &loss_rows})
+    if (t->has_value()) TORCH_CHECK((*t)->device() == logits16.device(), "outputs must be on the device of logits16");
+  b200::softmax_ce_soft_head(logits16.data_ptr(), ld, bias.data_ptr<float>(), labels.data_ptr<int64_t>(),
+                             mix.has_value() ? mix->data_ptr<int32_t>() : nullptr, (float)eps,
+                             logits32.has_value() ? logits32->data_ptr<float>() : nullptr,
+                             dlogits16.has_value() ? dlogits16->data_ptr() : nullptr,
+                             loss_rows.has_value() ? loss_rows->data_ptr<float>() : nullptr, stats.data_ptr<float>(), B,
+                             K, (float)grad_scale, cur());
+  after();
+}
 void fc_bias_grad(Tensor dlogits16, Tensor dbias) {
   chk(dlogits16, at::kBFloat16, "dlogits16");
   chk(dbias, at::kFloat, "dbias");
@@ -750,6 +796,54 @@ void augment_warp(Tensor x, Tensor out, Tensor params, std::string fill_mode, in
   after();
 }
 
+// augment_params plus the mix rows (int32 [N, 8]) of MixUp (mode 1) or CutMix (mode 2) in the same launch
+void augment_mix_params(Tensor params, Tensor mix, Tensor step, Tensor rot_table, Tensor lam_table, int64_t H, int64_t W,
+                        int64_t key, int64_t flip_mode, int64_t zq, int64_t txq, int64_t tyq, int64_t mode) {
+  TORCH_CHECK(params.dim() == 2 && params.size(0) >= 1, "params must be int32 [N, 8] with N >= 1");
+  aug_params_table(params, params.size(0), "params");
+  aug_params_table(mix, params.size(0), "mix");
+  TORCH_CHECK(mix.data_ptr() != params.data_ptr(), "mix and params must be separate buffers");
+  vec(step, at::kInt, 1, "step", 4);
+  vec(rot_table, at::kInt, 2 << b200::kAugRotBits, "rot_table", 8);
+  vec(lam_table, at::kInt, 2 << b200::kAugLamBits, "lam_table", 8);
+  for (const Tensor* t : {&mix, &step, &rot_table, &lam_table})
+    TORCH_CHECK(t->device() == params.device(), "mix, step, rot_table and lam_table must be on the device of params");
+  aug_side(H, W);
+  TORCH_CHECK(key >= 0 && key <= 0xFFFFFFFFLL, "key must be a uint32");
+  TORCH_CHECK(flip_mode >= 0 && flip_mode <= 3, "flip_mode: bit 0 horizontal, bit 1 vertical");
+  TORCH_CHECK(zq >= 0 && zq < 65536, "zq: Q16.16 zoom factor in [0, 1)");
+  TORCH_CHECK(txq >= 0 && txq <= W * 65536 && tyq >= 0 && tyq <= H * 65536,
+              "txq / tyq: Q16.16 translation in [0, W] / [0, H] pixels");
+  TORCH_CHECK(mode == b200::kMixUp || mode == b200::kCutMix, "mode: 1 MixUp, 2 CutMix");
+  b200::augment_mix_params(params.data_ptr<int32_t>(), mix.data_ptr<int32_t>(), step.data_ptr<int32_t>(),
+                           rot_table.data_ptr<int32_t>(), lam_table.data_ptr<int32_t>(), (int)params.size(0), (int)H,
+                           (int)W, (uint32_t)key, (int)flip_mode, (int32_t)zq, (int32_t)txq, (int32_t)tyq, (int)mode,
+                           cur());
+  after();
+}
+// out = augment_warp of x mixed with each image's partner by its mix row (mode 1 MixUp, 2 CutMix)
+void augment_mix_warp(Tensor x, Tensor out, Tensor params, Tensor mix, int64_t mode, std::string fill_mode,
+                      int64_t fill_value) {
+  chk(x, at::kByte, "x");
+  chk(out, at::kByte, "out");
+  TORCH_CHECK(x.dim() == 4 && x.size(3) == 3 && x.size(0) >= 1, "x must be uint8 [N, H, W, 3]");
+  TORCH_CHECK(out.sizes() == x.sizes(), "out must have the shape of x");
+  TORCH_CHECK(out.device() == x.device() && params.device() == x.device() && mix.device() == x.device(),
+              "x, out, params and mix must share a device");
+  TORCH_CHECK(out.data_ptr() != x.data_ptr(), "augment_mix_warp cannot run in place");
+  aligned(out, 16, "out");
+  aug_side(x.size(1), x.size(2));
+  aug_params_table(params, x.size(0), "params");
+  aug_params_table(mix, x.size(0), "mix");
+  TORCH_CHECK(mode == b200::kMixUp || mode == b200::kCutMix, "mode: 1 MixUp, 2 CutMix");
+  TORCH_CHECK(fill_mode == "reflect" || fill_mode == "constant", "fill_mode must be 'reflect' or 'constant'");
+  TORCH_CHECK(fill_value >= 0 && fill_value <= 255, "fill_value must be a uint8");
+  b200::augment_mix_warp(x.data_ptr<uint8_t>(), out.data_ptr<uint8_t>(), params.data_ptr<int32_t>(),
+                         mix.data_ptr<int32_t>(), (int)x.size(0), (int)x.size(1), (int)x.size(2), (int)mode,
+                         fill_mode == "reflect", (int)fill_value, cur());
+  after();
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -776,6 +870,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_ce_head", &softmax_ce_head, py::arg("logits16"), py::arg("bias"), py::arg("labels"),
         py::arg("logits32") = c10::nullopt, py::arg("dlogits16") = c10::nullopt, py::arg("loss_rows") = c10::nullopt,
         py::arg("stats"), py::arg("grad_scale") = 1.0);
+  m.def("softmax_ce_soft_head", &softmax_ce_soft_head, py::arg("logits16"), py::arg("bias"), py::arg("labels"),
+        py::arg("mix") = c10::nullopt, py::arg("label_smoothing") = 0.0, py::arg("logits32") = c10::nullopt,
+        py::arg("dlogits16") = c10::nullopt, py::arg("loss_rows") = c10::nullopt, py::arg("stats"),
+        py::arg("grad_scale") = 1.0);
   m.def("fc_bias_grad", &fc_bias_grad);
   m.def("pack_stem_weight", &pack_stem_weight);
   m.def("stem_pool_bn_bwd", &stem_pool_bn_bwd, py::arg("pass_"), py::arg("idx"), py::arg("g1"), py::arg("g2"), py::arg("y"),
@@ -818,4 +916,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("W"), py::arg("key"), py::arg("flip_mode"), py::arg("zq"), py::arg("txq"), py::arg("tyq"));
   m.def("augment_warp", &augment_warp, py::arg("x"), py::arg("out"), py::arg("params"), py::arg("fill_mode"),
         py::arg("fill_value"));
+  m.def("augment_mix_params", &augment_mix_params, py::arg("params"), py::arg("mix"), py::arg("step"),
+        py::arg("rot_table"), py::arg("lam_table"), py::arg("H"), py::arg("W"), py::arg("key"), py::arg("flip_mode"),
+        py::arg("zq"), py::arg("txq"), py::arg("tyq"), py::arg("mode"));
+  m.def("augment_mix_warp", &augment_mix_warp, py::arg("x"), py::arg("out"), py::arg("params"), py::arg("mix"),
+        py::arg("mode"), py::arg("fill_mode"), py::arg("fill_value"));
 }

@@ -16,11 +16,20 @@ Differences from Keras, on purpose:
 Parameters of image ``n`` at step ``t`` are a pure function of (seed, rank, t, n): draw ``k`` is
 ``hash_u32(key(seed, rank), t, 8 n + k)`` with the dropout hash (csrc/hash.cuh).  ``t`` is the optimizer's step counter,
 which checkpoints store, so a resumed run repeats the augmentation of an uninterrupted one.
+
+MixUp and CutMix (``mixup`` / ``cutmix``: the alpha of Keras's Beta(alpha, alpha)) mix every image with a partner of
+the same batch after the geometric warp, and the label weights travel to the soft-target head as integer mix rows.
+Draw 5 indexes a host-built table of 4096 Beta quantiles, draws 6 and 7 place the CutMix box, and one draw per step,
+``s = 1 + hash_u32(key, t, 8 N) mod (N - 1)``, gives ``partner(n) = (n + s) mod N``.  Differences from Keras:
+- The partners are a rotation of the batch (every image gets a different partner, and the rotation changes every step),
+  not a uniformly random permutation; each data-parallel rank mixes within its own batch.
+- lambda is one of 4096 quantiles of Beta(alpha, alpha), and MixUp weights are quantised to 1/256.
 """
 from __future__ import annotations
 
 import math
 from dataclasses import asdict, dataclass
+from functools import lru_cache
 from typing import Optional, Tuple
 
 import numpy as np
@@ -29,8 +38,12 @@ import torch
 FLIP_MODES = {None: 0, "horizontal": 1, "vertical": 2, "horizontal_and_vertical": 3}
 FILL_MODES = ("reflect", "constant")
 ROT_BITS = 12          # csrc/ops_api.h kAugRotBits: 4096 table angles
+LAM_BITS = 12          # csrc/ops_api.h kAugLamBits: 4096 Beta quantiles
 MAX_SIDE = 2048        # csrc/ops_api.h kAugMaxSide
 PARAM_FIELDS = 8       # a00 a01 b0 a10 a11 b1 flags 0
+MIX_FIELDS = 8         # partner, MixUp weight w, CutMix box x0 y0 x1 y1, mu = num / den
+MIX_NONE, MIX_UP, CUT_MIX = 0, 1, 2   # csrc/ops_api.h AugMix
+MAX_MIX_ALPHA = 100.0
 _M32 = 0xFFFFFFFF
 
 
@@ -40,7 +53,9 @@ class Augmentation:
     ``rotation`` f: angle uniform in [-2 pi f, 2 pi f], 0 <= f <= 0.5;  ``zoom`` z: sampling-grid scale uniform in
     [1 - z, 1 + z], 0 <= z < 1 (> 1 zooms out, as Keras);  ``translation`` f: x / y shifts independently uniform in
     [-f, f] of W / H, 0 <= f <= 1;  ``fill_mode``: "reflect" (d c b a | a b c d | d c b a) or "constant" with the uint8
-    ``fill_value``."""
+    ``fill_value``;  ``mixup`` / ``cutmix``: the alpha of Beta(alpha, alpha) for Keras's MixUp / CutMix, in [0, 100],
+    0 = off, at most one of them non-zero.  Mixing needs a loss that takes soft targets: the engines' head and the
+    module backend form them from the integer labels (see `train.losses.CategoricalCrossentropy`)."""
 
     flip: Optional[str] = None
     rotation: float = 0.0
@@ -48,6 +63,8 @@ class Augmentation:
     translation: float = 0.0
     fill_mode: str = "reflect"
     fill_value: int = 0
+    mixup: float = 0.0
+    cutmix: float = 0.0
 
     def __post_init__(self):
         if self.flip not in FLIP_MODES:
@@ -63,6 +80,14 @@ class Augmentation:
             raise ValueError(f"fill_mode must be one of {FILL_MODES}, got {self.fill_mode!r}")
         if isinstance(self.fill_value, bool) or not isinstance(self.fill_value, int) or not 0 <= self.fill_value <= 255:
             raise ValueError(f"fill_value must be an int in 0..255, got {self.fill_value!r}")
+        for name in ("mixup", "cutmix"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) \
+                    or not 0.0 <= v <= MAX_MIX_ALPHA:
+                raise ValueError(f"{name} must be a number in [0, {MAX_MIX_ALPHA:g}], got {v!r}")
+            object.__setattr__(self, name, float(v))
+        if self.mixup > 0 and self.cutmix > 0:
+            raise ValueError(f"mixup and cutmix cannot both be on (got mixup={self.mixup}, cutmix={self.cutmix})")
 
     def to_dict(self) -> dict:
         return asdict(self)
@@ -74,6 +99,20 @@ class Augmentation:
     @property
     def flip_mode(self) -> int:
         return FLIP_MODES[self.flip]
+
+    @property
+    def mix_mode(self) -> int:
+        """MIX_NONE, MIX_UP or CUT_MIX (csrc/ops_api.h AugMix)."""
+        return MIX_UP if self.mixup > 0 else CUT_MIX if self.cutmix > 0 else MIX_NONE
+
+    def lambda_table(self) -> torch.Tensor:
+        """int32 [4096, 2]: rint(65536 lambda_i) and rint(65536 sqrt(1 - lambda_i)) for the Beta(alpha, alpha)
+        quantiles lambda_i = I^-1((i + 0.5) / 4096; alpha, alpha), computed in float64 on the host."""
+        if self.mix_mode == MIX_NONE:
+            raise ValueError("lambda_table: neither mixup nor cutmix is on")
+        lam = beta_quantiles(self.mixup or self.cutmix, 1 << LAM_BITS)
+        tab = np.stack([np.rint(lam * 65536.0), np.rint(np.sqrt(1.0 - lam) * 65536.0)], 1)
+        return torch.from_numpy(tab.astype(np.int32))
 
     def quantised(self, H: int, W: int) -> Tuple[int, int, int]:
         """Q16.16 half-ranges (zoom, x translation in pixels, y translation in pixels) the kernels take."""
@@ -87,6 +126,59 @@ class Augmentation:
         theta = 2.0 * math.pi * self.rotation * (2.0 * np.arange(n, dtype=np.float64) - (n - 1)) / (n - 1)
         tab = np.stack([np.rint(np.cos(theta) * 65536.0), np.rint(np.sin(theta) * 65536.0)], 1)
         return torch.from_numpy(tab.astype(np.int32))
+
+
+# ------------------------------------------------------------------------------------------------ Beta quantiles
+def _betainc_lower(x: np.ndarray, a: float) -> np.ndarray:
+    """Regularised incomplete beta I_x(a, a) for 0 <= x <= 1/2 (float64), by its continued fraction (modified Lentz).
+    x <= 1/2 = (a + 1) / (2 a + 2) is the range where the fraction converges quickly."""
+    tiny = 1e-300
+    with np.errstate(divide="ignore"):
+        front = np.exp(a * (np.log(x) + np.log1p(-x)) - (2 * math.lgamma(a) - math.lgamma(2 * a))) / a
+    f = np.full_like(x, tiny)
+    C, D = f.copy(), np.zeros_like(x)
+    for j in range(1, 1000):
+        if j == 1:
+            num = np.ones_like(x)
+        elif j % 2 == 0:          # d_{2m+1}, m = (j - 2) / 2
+            m = (j - 2) // 2
+            num = -(a + m) * (2 * a + m) * x / ((a + 2 * m) * (a + 2 * m + 1))
+        else:                     # d_{2m}, m = (j - 1) / 2
+            m = (j - 1) // 2
+            num = m * (a - m) * x / ((a + 2 * m - 1) * (a + 2 * m))
+        D = 1.0 + num * D
+        D = np.where(D == 0, tiny, D)
+        C = 1.0 + num / C
+        C = np.where(C == 0, tiny, C)
+        D = 1.0 / D
+        delta = C * D
+        f = f * delta
+        if j > 2 and float(np.abs(delta - 1.0).max()) < 1e-15:
+            break
+    return front * f
+
+
+@lru_cache(maxsize=16)
+def _beta_quantiles(alpha: float, n: int) -> np.ndarray:
+    # Bisection of I_x(a, a) = p on [0, 1/2] for the lower half of the probabilities; the upper half mirrors it
+    # (Beta(a, a) is symmetric), so the table is exactly symmetric and monotone.
+    half = (n + 1) // 2
+    p = (np.arange(half, dtype=np.float64) + 0.5) / n
+    lo, hi = np.zeros(half), np.full(half, 0.5)
+    for _ in range(64):
+        mid = 0.5 * (lo + hi)
+        below = _betainc_lower(mid, alpha) < p
+        lo, hi = np.where(below, mid, lo), np.where(below, hi, mid)
+    x = 0.5 * (lo + hi)
+    out = np.empty(n)
+    out[:half] = x
+    out[n - half:] = 1.0 - x[::-1]
+    return out
+
+
+def beta_quantiles(alpha: float, n: int = 1 << LAM_BITS) -> np.ndarray:
+    """float64 [n]: the quantiles I^-1((i + 0.5) / n; alpha, alpha) of Beta(alpha, alpha), i = 0 .. n - 1."""
+    return _beta_quantiles(float(alpha), int(n)).copy()
 
 
 def check_augmentation(aug) -> Optional[Augmentation]:
@@ -188,21 +280,131 @@ def warp_reference(x_u8: torch.Tensor, params: torch.Tensor, fill_mode: str = "r
     return ((acc + 32768) >> 16).to(torch.uint8)
 
 
-def augment_reference(aug: Augmentation, x_u8: torch.Tensor, key: int, step: int) -> torch.Tensor:
-    """What the engines' training step feeds its stem: the warp of the uint8 NHWC batch at optimizer step ``step``."""
+def mix_params_reference(aug: Augmentation, N: int, H: int, W: int, key: int, step: int, device=None,
+                         lam_table: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The mix rows augment_mix_params writes: int32 [N, 8] = partner, MixUp weight w, CutMix box x0 y0 x1 y1 (half-open),
+    and the partner's label weight mu = num / den (see csrc/augment.cu)."""
+    mode = aug.mix_mode
+    if mode == MIX_NONE:
+        raise ValueError("mix_params_reference: neither mixup nor cutmix is on")
+    dev = torch.device(device) if device is not None else torch.device("cpu")
+    lam = (lam_table if lam_table is not None else aug.lambda_table()).to(dev, torch.int64)
+    n = torch.arange(N, device=dev, dtype=torch.int64)
+    c = n * 8
+    t = int(step) & 0x7FFFFFFF
+    shift = 1 + int(hash_u32(int(key), t, 8 * N)) % (N - 1) if N > 1 else 0
+    partner = (n + shift) % N
+    lq = lam[hash_u32(int(key), t, c + 5) >> (32 - LAM_BITS)]
+    zero = torch.zeros_like(n)
+    if mode == MIX_UP:
+        w = (lq[:, 0] + 128) >> 8
+        rows = [partner, w, zero, zero, zero, zero, 256 - w, torch.full_like(n, 256)]
+    else:
+        cx = (W * (hash_u32(int(key), t, c + 6) >> 16)) >> 16
+        cy = (H * (hash_u32(int(key), t, c + 7) >> 16)) >> 16
+        hw, hh = ((W * lq[:, 1] + 32768) >> 16) >> 1, ((H * lq[:, 1] + 32768) >> 16) >> 1
+        x0, x1 = (cx - hw).clamp(0, W), (cx + hw).clamp(0, W)
+        y0, y1 = (cy - hh).clamp(0, H), (cy + hh).clamp(0, H)
+        rows = [partner, zero, x0, y0, x1, y1, (x1 - x0) * (y1 - y0), torch.full_like(n, H * W)]
+    return torch.stack(rows, 1).to(torch.int32)
+
+
+def mix_warp_reference(x_u8: torch.Tensor, params: torch.Tensor, mix: torch.Tensor, mode: int,
+                       fill_mode: str = "reflect", fill_value: int = 0) -> torch.Tensor:
+    """augment_mix_warp: every image's geometric warp mixed with its partner's (``mode`` MIX_UP or CUT_MIX)."""
+    if mode not in (MIX_UP, CUT_MIX):
+        raise ValueError("mode must be MIX_UP or CUT_MIX")
+    N, H, W, _ = x_u8.shape
+    own = warp_reference(x_u8, params, fill_mode, fill_value).to(torch.int64)
+    m = mix.to(x_u8.device, torch.int64)
+    other = own[m[:, 0]]
+    if mode == MIX_UP:
+        w = m[:, 1].view(N, 1, 1, 1)
+        return ((w * own + (256 - w) * other + 128) >> 8).to(torch.uint8)
+    ys = torch.arange(H, device=x_u8.device).view(1, H, 1)
+    xs = torch.arange(W, device=x_u8.device).view(1, 1, W)
+    box = ((xs >= m[:, 2].view(N, 1, 1)) & (xs < m[:, 4].view(N, 1, 1)) & (ys >= m[:, 3].view(N, 1, 1))
+           & (ys < m[:, 5].view(N, 1, 1)))
+    return torch.where(box.unsqueeze(-1), other, own).to(torch.uint8)
+
+
+def augment_batch_reference(aug: Augmentation, x_u8: torch.Tensor, key: int, step: int):
+    """What the engines' training step feeds its stem and its head: the warp of the uint8 NHWC batch at optimizer step
+    ``step``, mixed with the partners' warps when MixUp or CutMix is on, and the mix rows (None without mixing)."""
     if x_u8.dtype != torch.uint8 or x_u8.dim() != 4 or x_u8.shape[3] != 3:
         raise ValueError(f"augmentation needs a uint8 [N, H, W, 3] batch, got {tuple(x_u8.shape)} {x_u8.dtype}")
     N, H, W, _ = x_u8.shape
     if max(H, W) > MAX_SIDE:
         raise ValueError(f"augmentation: image sides must be at most {MAX_SIDE}")
     params = params_reference(aug, N, H, W, key, step, device=x_u8.device)
-    return warp_reference(x_u8, params, aug.fill_mode, aug.fill_value)
+    if aug.mix_mode == MIX_NONE:
+        return warp_reference(x_u8, params, aug.fill_mode, aug.fill_value), None
+    mix = mix_params_reference(aug, N, H, W, key, step, device=x_u8.device)
+    return mix_warp_reference(x_u8, params, mix, aug.mix_mode, aug.fill_mode, aug.fill_value), mix
+
+
+def augment_reference(aug: Augmentation, x_u8: torch.Tensor, key: int, step: int) -> torch.Tensor:
+    """The batch of `augment_batch_reference` alone: what the engines' training step feeds its stem."""
+    return augment_batch_reference(aug, x_u8, key, step)[0]
+
+
+# ------------------------------------------------------------------------------------------------ soft targets
+def mix_weight(mix: Optional[torch.Tensor], B: int, device=None, dtype=torch.float32) -> torch.Tensor:
+    """mu = num / den of every mix row (0 without mixing), divided in ``dtype`` (float32: the head's __fdiv_rn)."""
+    if mix is None:
+        return torch.zeros(B, device=device, dtype=dtype)
+    m = mix.to(device)
+    return m[:, 6].to(dtype) / m[:, 7].to(dtype)
+
+
+def soft_targets(labels: torch.Tensor, num_classes: int, mix: Optional[torch.Tensor] = None,
+                 label_smoothing: float = 0.0, dtype=torch.float32) -> torch.Tensor:
+    """[B, K] targets of the soft-target head: (1 - eps) (lambda onehot(y_n) + mu onehot(y_partner)) + eps / K, with
+    lambda = 1 - mu."""
+    B = labels.numel()
+    y = labels.view(-1).long()
+    onehot = torch.nn.functional.one_hot(y, num_classes).to(dtype)
+    mu = mix_weight(mix, B, labels.device, dtype).view(B, 1)
+    t = onehot if mix is None else (1 - mu) * onehot + mu * onehot[mix[:, 0].to(labels.device).long()]
+    eps = float(label_smoothing)
+    return t if eps == 0 else (1 - eps) * t + eps / num_classes
+
+
+def target_argmax(labels: torch.Tensor, mix: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The class accuracy compares with: the argmax of the unsmoothed (mixed) target, lowest index on ties, decided on
+    the integers as the head does - the own label when 2 num < den, the partner's when 2 num > den, the lower of the two
+    on a tie.  Label smoothing does not enter: Keras applies it inside the loss, and its accuracy metric never sees it."""
+    y = labels.view(-1).long()
+    if mix is None:
+        return y
+    m = mix.to(y.device).long()
+    yp = y[m[:, 0]]
+    twice, den = 2 * m[:, 6], m[:, 7]
+    return torch.where(twice < den, y, torch.where(twice > den, yp, torch.minimum(y, yp)))
+
+
+def soft_head_reference(logits: torch.Tensor, labels: torch.Tensor, mix: Optional[torch.Tensor] = None,
+                        label_smoothing: float = 0.0, grad_scale: float = 1.0):
+    """float64 softmax_ce_soft_head of fp32 ``logits`` [B, K] (bias included): per-row losses
+    sum_k target_k (lse - logit_k), dlogits (p - target) * grad_scale, and the correct count
+    argmax(logits) == target_argmax(labels, mix) (lowest index on ties, for both)."""
+    z = logits.double()
+    K = z.shape[1]
+    t = soft_targets(labels, K, mix, label_smoothing, torch.float64)
+    lse = torch.logsumexp(z, 1, keepdim=True)
+    loss = (t * (lse - z)).sum(1)
+    d = (torch.softmax(z, 1) - t) * grad_scale
+    am = torch.from_numpy(np.argmax(logits.detach().cpu().numpy(), axis=1)).to(labels.device)
+    correct = int((am == target_argmax(labels, mix)).sum())
+    return loss, d, correct
 
 
 class DeviceAugmenter:
     """The two kernel launches of one engine: per-image parameters into ``params`` from the device step word, then the
     warp of ``x`` into ``out``.  The engine owns the buffers; the host writes the step word with `set_step` (a pinned
-    ring slot and an async copy, as the optimizer hyper-parameters are written), never as a kernel argument."""
+    ring slot and an async copy, as the optimizer hyper-parameters are written), never as a kernel argument.  With
+    MixUp or CutMix the same two launches also write the mix rows ``mix`` (the soft-target head reads them) and mix
+    every image with its partner; without, ``mix`` is None."""
 
     def __init__(self, aug: Augmentation, x: torch.Tensor, seed: int, rank: int = 0):
         from .. import ops
@@ -221,6 +423,10 @@ class DeviceAugmenter:
         self.key = augment_key(seed, rank)
         self._zq, self._txq, self._tyq = aug.quantised(H, W)
         self._upload = PinnedUpload(self.step)
+        self.mix = None
+        if aug.mix_mode != MIX_NONE:
+            self.mix = torch.zeros(N, MIX_FIELDS, device=x.device, dtype=torch.int32)
+            self.lam_table = aug.lambda_table().to(x.device)
 
     def set_step(self, t: int) -> None:
         """Host -> device write of the step word (outside any CUDA graph; the graph reads it on replay)."""
@@ -231,11 +437,19 @@ class DeviceAugmenter:
     def run_params(self) -> None:
         """augment_params: the per-image transforms of the step in the device step word."""
         _, H, W, _ = self.x.shape
+        if self.mix is not None:
+            self._e.augment_mix_params(self.params, self.mix, self.step, self.rot_table, self.lam_table, H, W, self.key,
+                                       self.aug.flip_mode, self._zq, self._txq, self._tyq, self.aug.mix_mode)
+            return
         self._e.augment_params(self.params, self.step, self.rot_table, H, W, self.key, self.aug.flip_mode, self._zq,
                                self._txq, self._tyq)
 
     def run_warp(self) -> None:
-        """augment_warp: ``out`` = the batch resampled by the transforms in ``params``."""
+        """augment_warp: ``out`` = the batch resampled by the transforms in ``params`` (and mixed by ``mix``)."""
+        if self.mix is not None:
+            self._e.augment_mix_warp(self.x, self.out, self.params, self.mix, self.aug.mix_mode, self.aug.fill_mode,
+                                     self.aug.fill_value)
+            return
         self._e.augment_warp(self.x, self.out, self.params, self.aug.fill_mode, self.aug.fill_value)
 
     def run(self) -> None:

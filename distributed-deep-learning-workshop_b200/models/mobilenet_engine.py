@@ -74,6 +74,8 @@ class MobileNetV2Engine:
         ops.require_native()
         self.augmentation = check_augmentation(augmentation)
         self._augmenter = None
+        # Keras's label smoothing of the loss; the Trainer sets it from the compiled loss before capturing the steps
+        self.label_smoothing = 0.0
         if image_size % 32:
             raise ValueError("image_size must be a multiple of 32")
         check_fine_tune_at(fine_tune_at)
@@ -548,8 +550,14 @@ class MobileNetV2Engine:
         e.gap_fwd(self.feat, self.pooled, drop, self._drop_seed)
         self._fc_fwd.run()
         e.zero_(self.stats)
-        e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits,
-                          self.dlogits16 if (training and self._training_built) else None, self.loss_rows, self.stats, 1.0 / N)
+        dl = self.dlogits16 if (training and self._training_built) else None
+        mix = self._augmenter.mix if (training and self._augmenter is not None) else None
+        if mix is None and self.label_smoothing == 0:
+            e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits, dl, self.loss_rows,
+                              self.stats, 1.0 / N)
+        else:   # soft targets: the partner's label at the mix row's weight, label smoothing
+            e.softmax_ce_soft_head(self.logits16, self.p("fc.bias"), self.labels, mix, self.label_smoothing,
+                                   self.logits, dl, self.loss_rows, self.stats, 1.0 / N)
 
     def backward(self) -> None:
         """Dense head weight / bias gradients; with fine_tune_at <= 18 also those of base.features[fine_tune_at:]."""

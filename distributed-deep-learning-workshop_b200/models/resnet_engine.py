@@ -107,6 +107,8 @@ class ResNet50Engine:
         ops.require_native()
         self.augmentation = check_augmentation(augmentation)
         self._augmenter = None
+        # Keras's label smoothing of the loss; the Trainer sets it from the compiled loss before capturing the steps
+        self.label_smoothing = 0.0
         self.zero_init_residual = zero_init_residual
         self.native_stem = native_stem
         # experimental: run every weight-gradient GEMM on a side stream so it overlaps the (DRAM-bound) BatchNorm
@@ -652,9 +654,16 @@ class ResNet50Engine:
         e.gap_fwd(self.feat, self.pooled, drop, self._drop_seed)
         self._fc_fwd.run()  # bf16 logits (class dimension padded) on the wgmma GEMM
         e.zero_(self.stats)
-        # + bias, softmax cross-entropy, accuracy, bf16 dlogits (padded columns zero) in one kernel
-        e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits,
-                          self.dlogits16 if training else None, self.loss_rows, self.stats, 1.0 / N)
+        # + bias, softmax cross-entropy, accuracy, bf16 dlogits (padded columns zero) in one kernel; against the soft
+        # target when the batch is mixed or the labels smoothed
+        mix = self._augmenter.mix if (training and self._augmenter is not None) else None
+        if mix is None and self.label_smoothing == 0:
+            e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits,
+                              self.dlogits16 if training else None, self.loss_rows, self.stats, 1.0 / N)
+        else:   # soft targets: the partner's label at the mix row's weight, label smoothing
+            e.softmax_ce_soft_head(self.logits16, self.p("fc.bias"), self.labels, mix, self.label_smoothing,
+                                   self.logits, self.dlogits16 if training else None, self.loss_rows, self.stats,
+                                   1.0 / N)
 
     # ------------------------------------------------------------------------------------------------ backward
     def _ready(self, *names: str) -> None:

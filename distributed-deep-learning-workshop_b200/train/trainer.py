@@ -28,10 +28,12 @@ def _is_engine(model) -> bool:
 
 
 class _EngineBackend:
-    def __init__(self, engine, optimizer, use_graph: bool):
+    def __init__(self, engine, optimizer, use_graph: bool, label_smoothing: float = 0.0):
         from ..models.resnet_engine import EngineTrainStep, EngineEvalStep
 
         self.engine = engine
+        # read by the head of every forward: set before the (lazily built) steps capture their graphs
+        engine.label_smoothing = float(label_smoothing)
         self.optimizer = optimizer
         self.use_graph = use_graph
         # Both step objects are created on first use: a Trainer that only ever predicts (pyfunc serving, load_model) builds
@@ -164,8 +166,10 @@ class _EngineBackend:
 
 
 class _ModuleBackend:
-    def __init__(self, module: torch.nn.Module, optimizer, preprocess, device: torch.device):
+    def __init__(self, module: torch.nn.Module, optimizer, preprocess, device: torch.device,
+                 label_smoothing: float = 0.0):
         self.module = module.to(device)
+        self.label_smoothing = float(label_smoothing)
         self.device = device
         self.optimizer = optimizer
         self.preprocess = preprocess
@@ -185,40 +189,49 @@ class _ModuleBackend:
         x = torch.as_tensor(x).to(self.device, non_blocking=True)
         return self.preprocess(x)
 
-    def _augmented(self, x) -> torch.Tensor:
-        """The uint8 NHWC batch warped by ``module.augmentation`` at the optimizer's current step (the reference
-        implementation of the engines' augmentation kernels, same draws for the same seed, rank and step)."""
-        from ..models.augment import augment_key, augment_reference
+    def _augmented(self, x):
+        """The uint8 NHWC batch warped (and mixed) by ``module.augmentation`` at the optimizer's current step, and the
+        mix rows (None without MixUp / CutMix): the reference implementation of the engines' augmentation kernels, same
+        draws for the same seed, rank and step."""
+        from ..models.augment import augment_batch_reference, augment_key
 
         x = torch.as_tensor(x)
         if x.dtype != torch.uint8:
             raise ValueError(f"augmentation needs the uint8 [N, H, W, 3] batch, got {x.dtype}")
         opt = self.optimizer.opt if hasattr(self.optimizer, "opt") else self.optimizer
         key = augment_key(getattr(self.module, "augmentation_seed", 0), dist_core.rank())
-        return augment_reference(self.module.augmentation, x.to(self.device, non_blocking=True), key, opt.t)
+        return augment_batch_reference(self.module.augmentation, x.to(self.device, non_blocking=True), key, opt.t)
 
     def train_batch(self, x, y) -> None:
+        from ..models.augment import soft_targets, target_argmax
+
         self.module.train()
         y = torch.as_tensor(y).to(self.device, non_blocking=True)
         self.optimizer.begin_step()
+        mix = None
         if getattr(self.module, "augmentation", None) is not None:
-            x = self._augmented(x)
+            x, mix = self._augmented(x)
         self.flat.zero_grad()
         if self._dist:
             self.optimizer.start_backward()
         logits = self.module(self._prep(x)).float()
-        loss = torch.nn.functional.cross_entropy(logits, y)
+        eps = self.label_smoothing
+        if mix is None and eps == 0:
+            loss = torch.nn.functional.cross_entropy(logits, y)
+            acc = (logits.argmax(1) == y).float().mean()
+        else:
+            loss = torch.nn.functional.cross_entropy(logits, soft_targets(y, logits.shape[1], mix, eps))
+            acc = (logits.argmax(1) == target_argmax(y, mix)).float().mean()
         loss.backward()
         self.optimizer.step()
-        acc = (logits.argmax(1) == y).float().mean()
-        self._results.append(torch.stack([loss.detach(), acc]))
+        self._results.append(torch.stack([loss.detach(), acc.detach()]))
 
     @torch.no_grad()
     def eval_batch(self, x, y) -> None:
         self.module.eval()
         y = torch.as_tensor(y).to(self.device, non_blocking=True)
         logits = self.module(self._prep(x)).float()
-        loss = torch.nn.functional.cross_entropy(logits, y)
+        loss = torch.nn.functional.cross_entropy(logits, y, label_smoothing=self.label_smoothing)
         acc = (logits.argmax(1) == y).float().mean()
         self._results.append(torch.stack([loss, acc]))
 
@@ -274,20 +287,27 @@ class Trainer:
     def compile(self, optimizer, loss: str = "sparse_categorical_crossentropy", metrics: Sequence[str] = ("accuracy",),
                 **_ignored) -> "Trainer":
         """`model.compile(optimizer=..., loss=SparseCategoricalCrossentropy(from_logits=True), metrics=['accuracy'])`;
-        ``optimizer`` may be a name (``"rmsprop"``, ``"adamw"``, ...): `optim.get(name)()` with Keras's defaults."""
+        ``optimizer`` may be a name (``"rmsprop"``, ``"adamw"``, ...): `optim.get(name)()` with Keras's defaults.
+        ``loss`` may also be `losses.CategoricalCrossentropy(from_logits=True, label_smoothing=eps)` or
+        ``"categorical_crossentropy"``, which a model whose augmentation uses MixUp or CutMix requires."""
         if isinstance(optimizer, str):
             from .. import optim
 
             optimizer = optim.get(optimizer)()
-        loss_name = loss if isinstance(loss, str) else getattr(loss, "name", "sparse_categorical_crossentropy")
-        if "sparse_categorical_crossentropy" not in loss_name:
-            raise ValueError("only sparse categorical cross-entropy from logits is implemented (what the reference uses)")
+        from .losses import CategoricalCrossentropy, label_smoothing_of
+
+        eps = label_smoothing_of(loss)
+        aug = getattr(self.model, "augmentation", None)
+        if aug is not None and aug.mix_mode and not (isinstance(loss, CategoricalCrossentropy)
+                                                     or loss == "categorical_crossentropy"):
+            raise ValueError("MixUp / CutMix train on soft targets: compile with "
+                             "CategoricalCrossentropy(from_logits=True) or 'categorical_crossentropy'")
         self.optimizer = optimizer
         self.metrics_names = ["loss"] + [m if isinstance(m, str) else getattr(m, "name", "metric") for m in metrics]
         if _is_engine(self.model):
-            self.backend = _EngineBackend(self.model, optimizer, self.use_graph)
+            self.backend = _EngineBackend(self.model, optimizer, self.use_graph, eps)
         else:
-            self.backend = _ModuleBackend(self.model, optimizer, self._preprocess, self.device)
+            self.backend = _ModuleBackend(self.model, optimizer, self._preprocess, self.device, eps)
         return self
 
     # ------------------------------------------------------------------------------------------------ fit
@@ -428,7 +448,9 @@ class Trainer:
     def _compile_for_inference(self) -> None:
         from .. import optim
 
-        self.compile(optim.SGD(0.0))
+        # an inference compile never trains, so a mixing augmentation's need for soft targets does not apply; without
+        # smoothing the categorical loss evaluates exactly as the sparse one
+        self.compile(optim.SGD(0.0), loss="categorical_crossentropy")
         if hasattr(self.backend, "inference_only"):
             self.backend.inference_only = True  # engine backend: build with the fused inference epilogues
 
