@@ -16,7 +16,8 @@
 //   k = 1: rotation table index (top 12 bits)     k = 2: zoom        k = 3 / 4: x / y translation   (top 16 bits)
 //   k = 5: lambda table index (top 12 bits)       k = 6 / 7: CutMix box centre x / y (top 16 bits)
 // and the batch's partner rotation is hash_u32(key, step, 8 N).  With MixUp or CutMix on, augment_mix_params and
-// augment_mix_warp take the places of augment_params and augment_warp: still two launches.
+// augment_mix_warp take the places of augment_params and augment_warp: still two launches.  Color augmentation adds a
+// third, augment_color, in place on the warp's output (or alone, from the raw batch, when nothing else is on).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -322,6 +323,281 @@ void augment_mix_warp(const uint8_t* x, uint8_t* out, const int32_t* params, con
     launch_mix_warp<kMixUp>(x, out, params, mix, N, H, W, reflect, fill, s);
   else
     launch_mix_warp<kCutMix>(x, out, params, mix, N, H, W, reflect, fill, s);
+}
+
+// ------------------------------------------------------------------------------------------------ color
+// Brightness, contrast, saturation, hue and grayscale of every image, in that order, on the batch the warp wrote (in
+// place) or on the raw batch.  Every channel value is v = 256 p (Q8) in int32 / int64; v is clamped to [0, 255 * 256]
+// after brightness and after contrast and rounded once at the end, (v + 128) >> 8.  Draw k of image n is
+// hash_u32(ckey, step, 8 n + k) with ckey = hash_u32(key, 0x436F6C72, 0) (models/augment.py color_key), so the
+// geometric and mix draws are untouched:
+//   k = 0: brightness delta  -bq + floor(2 bq u / 2^16)           (Q8 levels)
+//   k = 1: contrast factor   f = 1 - cq + floor(2 cq u / 2^16)    (Q16)
+//   k = 2: saturation factor S, likewise from sq                  (Q16)
+//   k = 3: hue shift         -hq + floor(2 hq u / 2^16)           (Q16 sixths of a turn)
+//   k = 4: grayscale         u < pq                               (u = top 16 bits of the draw)
+// A stage whose half-range is 0 is skipped, not computed as an identity.
+//
+// One cluster of G CTAs per image (G in 1, 2, 4, 8).  The image's 16-pixel groups that start on a 16-pixel boundary
+// of the flattened batch (48 bytes: three 16-byte accesses) are split into G contiguous slices; the pixels before the
+// first and after the last whole group go byte by byte to ranks 0 and G - 1.  With contrast on, each CTA first sums
+// its slice's post-brightness values into three uint64 partials in shared memory; after barrier.cluster every CTA adds
+// the G partials in rank order over DSMEM, so every CTA holds the same exact sums and means, and applies the chain to
+// its own slice (a slice is read twice; the second read is meant to come from L2).  A CTA arrives on a second cluster barrier after its DSMEM reads
+// and waits on it before exiting, so no shared memory is released while a peer may still read it.  Without contrast
+// there is no reduction and no barrier.
+constexpr int kColorThreads = 256;
+constexpr int kColorMax = 255 * 256;              // Q8 ceiling of a channel
+constexpr uint32_t kGrayR = 19589, kGrayG = 38470, kGrayB = 7471;   // rint(65536 x (0.2989, 0.5870, 0.1140))
+enum ColorStage : int { kBright = 1, kContrast = 2, kSaturate = 4, kHue = 8, kGray = 16 };
+
+struct ColorImage {
+  int flags, delta, f, sat, dh;
+  int mean[3];
+};
+
+// uniform in [-q, q) on a 2^-16 grid from the top 16 bits of a draw
+__device__ __forceinline__ int color_uniform(uint32_t r, int32_t q) {
+  return -q + (int)((2 * (int64_t)q * (int64_t)(r >> 16)) >> 16);
+}
+
+__device__ __forceinline__ int clamp_q8(int v) { return min(max(v, 0), kColorMax); }
+
+// Q16 fraction a / dl of a sixth of a turn, rounded half up (0 <= a <= dl; a 65536 + dl / 2 < 2^32)
+__device__ __forceinline__ int hue_frac(int a, uint32_t dl) {
+  return (int)(((uint32_t)a * 65536u + (dl >> 1)) / dl);
+}
+
+// Saturation, hue and grayscale of one Q8 pixel (brightness and contrast come before, per channel).
+__device__ __forceinline__ void color_hsv(int& r, int& g, int& b, const ColorImage& ci) {
+  if (ci.flags & kSaturate) {
+    // v' = mx - (mx - v) k, k = min(S, mx / dl): value (the max) kept, saturation dl / mx scaled by k and capped at
+    // 1.  S <= 1 already satisfies the cap (mx >= dl), so the division only runs above 1.  (mx - v) k <= mx 2^16.
+    const int mx = max(r, max(g, b)), dl = mx - min(r, min(g, b));
+    if (dl > 0) {
+      const uint32_t k = ci.sat <= 65536 ? (uint32_t)ci.sat : min((uint32_t)ci.sat, ((uint32_t)mx << 16) / (uint32_t)dl);
+      r = mx - (int)(((uint32_t)(mx - r) * k + 32768u) >> 16);
+      g = mx - (int)(((uint32_t)(mx - g) * k + 32768u) >> 16);
+      b = mx - (int)(((uint32_t)(mx - b) * k + 32768u) >> 16);
+    }
+  }
+  if (ci.flags & kHue) {
+    // hue position P in Q16 sixths of a turn (the max channel taken in the order R, G, B), rotated by dh; the pixel
+    // is rebuilt from (sector, fraction) with its max and min kept
+    const int mx = max(r, max(g, b)), mn = min(r, min(g, b));
+    const uint32_t dl = (uint32_t)(mx - mn);
+    if (dl > 0) {
+      // P = base + (a / dl) sixths, a signed: (g - b) / dl around R, 2 + (b - r) / dl around G, 4 + (r - g) / dl
+      // around B; |a| is rounded, so one division serves every branch
+      const int a = r == mx ? g - b : g == mx ? b - r : r - g;
+      const int base = r == mx ? 0 : g == mx ? 2 * 65536 : 4 * 65536;
+      const int q = hue_frac(abs(a), dl);
+      int P = base + (a < 0 ? -q : q);
+      P = (P + ci.dh + 12 * 65536) % (6 * 65536);
+      const int part = (int)(((uint32_t)(P & 65535) * dl + 32768u) >> 16);
+      const int rise = mn + part, fall = mx - part;
+      switch (P >> 16) {
+        case 0: r = mx; g = rise; b = mn; break;
+        case 1: r = fall; g = mx; b = mn; break;
+        case 2: r = mn; g = mx; b = rise; break;
+        case 3: r = mn; g = fall; b = mx; break;
+        case 4: r = rise; g = mn; b = mx; break;
+        default: r = mx; g = mn; b = fall; break;
+      }
+    }
+  }
+  if (ci.flags & kGray) {
+    r = g = b = (int)((kGrayR * (uint32_t)r + kGrayG * (uint32_t)g + kGrayB * (uint32_t)b + 32768u) >> 16);
+  }
+}
+
+__device__ __forceinline__ int color_bright(int p, const ColorImage& ci) {
+  return (ci.flags & kBright) ? clamp_q8((p << 8) + ci.delta) : p << 8;
+}
+
+// The whole chain on one pixel's three bytes.
+__device__ __forceinline__ void color_pixel(int (&p)[3], const ColorImage& ci) {
+  int v[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    v[c] = color_bright(p[c], ci);
+    if (ci.flags & kContrast)
+      v[c] = clamp_q8(ci.mean[c] + (int)(((int64_t)(v[c] - ci.mean[c]) * ci.f + 32768) >> 16));
+  }
+  color_hsv(v[0], v[1], v[2], ci);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) p[c] = (v[c] + 128) >> 8;
+}
+
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+// a uint64 in the shared memory of CTA `rank` of the cluster, at the offset of `p` in this CTA's
+__device__ __forceinline__ uint64_t ld_dsmem_u64(const uint64_t* p, uint32_t rank) {
+  const uint32_t local = (uint32_t)__cvta_generic_to_shared(p);
+  uint32_t remote;
+  uint64_t v;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(rank));
+  asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(v) : "r"(remote) : "memory");
+  return v;
+}
+
+__device__ __forceinline__ uint32_t byte_of(const uint32_t (&w)[12], int j) { return (w[j >> 2] >> ((j & 3) * 8)) & 255u; }
+
+__global__ void __launch_bounds__(kColorThreads, 4)
+augment_color_kernel(const uint8_t* src, uint8_t* dst, const int32_t* __restrict__ step, int HW, uint32_t ckey,
+                     int32_t bq, int32_t cq, int32_t sq, int32_t hq, int32_t pq) {
+  __shared__ uint64_t partial[3];
+  __shared__ uint64_t warp_sum[kColorThreads / 32][3];
+  __shared__ int mean_s[3];
+  const int G = (int)cluster_nctarank(), rank = (int)cluster_ctarank();
+  const int n = blockIdx.x / G;
+  const uint32_t t = (uint32_t)*step, c8 = (uint32_t)n * 8u;
+
+  ColorImage ci;
+  ci.flags = (bq ? kBright : 0) | (cq ? kContrast : 0) | (sq ? kSaturate : 0) | (hq ? kHue : 0);
+  ci.delta = bq ? color_uniform(hash_u32(ckey, t, c8), bq) : 0;
+  ci.f = cq ? 65536 + color_uniform(hash_u32(ckey, t, c8 + 1), cq) : 65536;
+  ci.sat = sq ? 65536 + color_uniform(hash_u32(ckey, t, c8 + 2), sq) : 65536;
+  ci.dh = hq ? color_uniform(hash_u32(ckey, t, c8 + 3), hq) : 0;
+  if (pq && (int32_t)(hash_u32(ckey, t, c8 + 4) >> 16) < pq) ci.flags |= kGray;
+
+  // global pixel range of the image, its whole 16-pixel groups [g0, g1) and this CTA's share of them
+  const int64_t a = (int64_t)n * HW, e = a + HW;
+  const int64_t g0 = (a + 15) >> 4, g1 = max(e >> 4, g0);
+  const int64_t head_end = min(g0 * 16, e), tail_begin = max(g1 * 16, head_end);
+  const int64_t ng = g1 - g0;
+  const int64_t gs = g0 + ng * rank / G, ge = g0 + ng * (rank + 1) / G;
+  const int64_t sa = rank == 0 ? a : 0, sb = rank == 0 ? head_end : 0;                 // single pixels of this CTA
+  const int64_t ta = rank == G - 1 ? tail_begin : 0, tb = rank == G - 1 ? e : 0;
+  const int tid = threadIdx.x;
+
+  if (ci.flags & kContrast) {
+    uint64_t s0 = 0, s1 = 0, s2 = 0;
+    for (int64_t i = gs + tid; i < ge; i += kColorThreads) {
+      const uint4* p = reinterpret_cast<const uint4*>(src + i * 48);
+      const uint4 q0 = p[0], q1 = p[1], q2 = p[2];
+      const uint32_t w[12] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w};
+      uint32_t u[3] = {0, 0, 0};   // 16 values of at most 255 * 256 each
+#pragma unroll
+      for (int j = 0; j < 48; ++j) u[j % 3] += (uint32_t)color_bright((int)byte_of(w, j), ci);
+      s0 += u[0]; s1 += u[1]; s2 += u[2];
+    }
+    for (int64_t P = sa + tid; P < sb; P += kColorThreads) {
+      s0 += (uint32_t)color_bright(src[3 * P], ci);
+      s1 += (uint32_t)color_bright(src[3 * P + 1], ci);
+      s2 += (uint32_t)color_bright(src[3 * P + 2], ci);
+    }
+    for (int64_t P = ta + tid; P < tb; P += kColorThreads) {
+      s0 += (uint32_t)color_bright(src[3 * P], ci);
+      s1 += (uint32_t)color_bright(src[3 * P + 1], ci);
+      s2 += (uint32_t)color_bright(src[3 * P + 2], ci);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+      s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    if ((tid & 31) == 0) {
+      warp_sum[tid >> 5][0] = s0;
+      warp_sum[tid >> 5][1] = s1;
+      warp_sum[tid >> 5][2] = s2;
+    }
+    __syncthreads();
+    if (tid < 3) {
+      uint64_t s = 0;
+      for (int w = 0; w < kColorThreads / 32; ++w) s += warp_sum[w][tid];
+      partial[tid] = s;
+    }
+    cluster_arrive();   // partials visible to the cluster
+    cluster_wait();
+    if (tid < 3) {
+      uint64_t s = 0;
+      for (int q = 0; q < G; ++q) s += ld_dsmem_u64(&partial[tid], (uint32_t)q);
+      mean_s[tid] = (int)((s + (uint64_t)(HW >> 1)) / (uint64_t)HW);
+    }
+    __syncthreads();
+    cluster_arrive();   // this CTA is done reading its peers; it waits for theirs before exiting
+    ci.mean[0] = mean_s[0];
+    ci.mean[1] = mean_s[1];
+    ci.mean[2] = mean_s[2];
+  } else {
+    ci.mean[0] = ci.mean[1] = ci.mean[2] = 0;
+  }
+
+  for (int64_t i = gs + tid; i < ge; i += kColorThreads) {
+    const uint4* p = reinterpret_cast<const uint4*>(src + i * 48);
+    const uint4 q0 = __ldcs(p), q1 = __ldcs(p + 1), q2 = __ldcs(p + 2);
+    const uint32_t w[12] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w};
+    uint32_t o[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) o[k] = 0;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      int px[3] = {(int)byte_of(w, 3 * j), (int)byte_of(w, 3 * j + 1), (int)byte_of(w, 3 * j + 2)};
+      color_pixel(px, ci);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) o[(3 * j + c) >> 2] |= (uint32_t)px[c] << (((3 * j + c) & 3) * 8);
+    }
+    uint4* d = reinterpret_cast<uint4*>(dst + i * 48);
+    d[0] = make_uint4(o[0], o[1], o[2], o[3]);
+    d[1] = make_uint4(o[4], o[5], o[6], o[7]);
+    d[2] = make_uint4(o[8], o[9], o[10], o[11]);
+  }
+  for (int half = 0; half < 2; ++half) {
+    const int64_t lo = half ? ta : sa, hi = half ? tb : sb;
+    for (int64_t P = lo + tid; P < hi; P += kColorThreads) {
+      int px[3] = {src[3 * P], src[3 * P + 1], src[3 * P + 2]};
+      color_pixel(px, ci);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) dst[3 * P + c] = (uint8_t)px[c];
+    }
+  }
+  if (ci.flags & kContrast) cluster_wait();
+}
+
+int augment_color(const uint8_t* src, uint8_t* dst, const int32_t* step, int N, int H, int W, uint32_t ckey, int32_t bq,
+                  int32_t cq, int32_t sq, int32_t hq, int32_t pq, int cluster, cudaStream_t s) {
+  // G: the smallest cluster that gives at least two waves of resident CTAs (at most 8), so a batch of a few dozen
+  // images still spreads over every SM, and CTAs waiting at the cluster barrier leave room for others to run
+  static int resident = 0;
+  if (resident == 0) {
+    int dev = 0, sms = 0, per_sm = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, augment_color_kernel, kColorThreads, 0);
+    resident = sms * per_sm > 0 ? sms * per_sm : 132 * 4;
+  }
+  int G = cluster;
+  if (G == 0) {
+    G = 1;
+    while (G < kAugColorMaxCluster && (int64_t)N * G < 2 * (int64_t)resident) G *= 2;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(N * G));
+  cfg.blockDim = dim3(kColorThreads);
+  cfg.dynamicSmemBytes = 0;
+  cfg.stream = s;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = (unsigned)G;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (cudaLaunchKernelEx(&cfg, augment_color_kernel, src, dst, step, H * W, ckey, bq, cq, sq, hq, pq) != cudaSuccess)
+    return -1;
+  return G;
 }
 
 }  // namespace b200

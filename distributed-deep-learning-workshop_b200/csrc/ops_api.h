@@ -169,6 +169,14 @@ void augment_mix_params(int32_t* params, int32_t* mix, const int32_t* step, cons
                         int32_t txq, int32_t tyq, int mode, cudaStream_t s);
 void augment_mix_warp(const uint8_t* x, uint8_t* out, const int32_t* params, const int32_t* mix, int N, int H, int W,
                       int mode, bool reflect, int fill, cudaStream_t s);
+// Color augmentation on top of the warp (or of the raw batch), in place or not: brightness, contrast, saturation, hue,
+// grayscale in that order, in Q8 fixed point.  Half-ranges: bq Q8 levels (<= 255 * 256), cq / sq Q16 (<= 65536),
+// hq Q16 sixths of a turn (<= 3 * 65536), pq Q16 grayscale probability (<= 65536); 0 skips the stage.  ckey: the
+// color draw key.  cluster: CTAs per image (1, 2, 4 or 8; 0 = chosen from N and the SM count); the bytes do not
+// depend on it.  Returns the cluster size launched.
+constexpr int kAugColorMaxCluster = 8;
+int augment_color(const uint8_t* src, uint8_t* dst, const int32_t* step, int N, int H, int W, uint32_t ckey, int32_t bq,
+                  int32_t cq, int32_t sq, int32_t hq, int32_t pq, int cluster, cudaStream_t s);
 // softmax_ce_head against the soft target (1 - eps) (lambda [k = y_n] + mu [k = y_partner]) + eps / K; mix may be
 // nullptr (mu = 0: label smoothing alone)
 void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const int64_t* labels, const int32_t* mix,

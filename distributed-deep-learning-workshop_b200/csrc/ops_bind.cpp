@@ -844,6 +844,43 @@ void augment_mix_warp(Tensor x, Tensor out, Tensor params, Tensor mix, int64_t m
   after();
 }
 
+// dst = color augmentation of src (uint8 [N, H, W, 3]; dst may be src) for the step held in `step`; returns the number
+// of CTAs per image launched (`cluster`: 1, 2, 4 or 8, or 0 to let the launch choose; the bytes do not depend on it)
+int64_t augment_color(Tensor src, Tensor dst, Tensor step, int64_t H, int64_t W, int64_t ckey, int64_t bq, int64_t cq,
+                      int64_t sq, int64_t hq, int64_t pq, int64_t cluster) {
+  chk(src, at::kByte, "src");
+  chk(dst, at::kByte, "dst");
+  TORCH_CHECK(src.dim() == 4 && src.size(3) == 3 && src.size(0) >= 1, "src must be uint8 [N, H, W, 3]");
+  TORCH_CHECK(src.size(1) == H && src.size(2) == W, "src must be [N, H, W, 3] for the given H and W");
+  TORCH_CHECK(dst.sizes() == src.sizes(), "dst must have the shape of src");
+  aug_side(H, W);
+  TORCH_CHECK(src.size(0) * b200::kAugColorMaxCluster < (1LL << 31), "augment_color: batch too large");
+  aligned(src, 16, "src");
+  aligned(dst, 16, "dst");
+  const bool same = src.data_ptr() == dst.data_ptr();
+  if (!same) {   // in place is allowed; a partial overlap is not
+    const auto s0 = reinterpret_cast<uintptr_t>(src.data_ptr()), d0 = reinterpret_cast<uintptr_t>(dst.data_ptr());
+    const auto nb = (uintptr_t)src.numel();
+    TORCH_CHECK(s0 + nb <= d0 || d0 + nb <= s0, "augment_color: src and dst overlap without being the same buffer");
+  }
+  vec(step, at::kInt, 1, "step", 4);
+  TORCH_CHECK(dst.device() == src.device() && step.device() == src.device(), "src, dst and step must share a device");
+  TORCH_CHECK(ckey >= 0 && ckey <= 0xFFFFFFFFLL, "ckey must be a uint32");
+  TORCH_CHECK(bq >= 0 && bq <= 255 * 256, "bq: Q8 brightness half-range in [0, 255 * 256]");
+  TORCH_CHECK(cq >= 0 && cq <= 65536, "cq: Q16 contrast half-range in [0, 1]");
+  TORCH_CHECK(sq >= 0 && sq <= 65536, "sq: Q16 saturation half-range in [0, 1]");
+  TORCH_CHECK(hq >= 0 && hq <= 3 * 65536, "hq: Q16 hue half-range in [0, 3] sixths of a turn");
+  TORCH_CHECK(pq >= 0 && pq <= 65536, "pq: Q16 grayscale probability in [0, 1]");
+  TORCH_CHECK(cluster == 0 || cluster == 1 || cluster == 2 || cluster == 4 || cluster == 8,
+              "cluster must be 0 (chosen by the launch), 1, 2, 4 or 8");
+  const int G = b200::augment_color(src.data_ptr<uint8_t>(), dst.data_ptr<uint8_t>(), step.data_ptr<int32_t>(),
+                                    (int)src.size(0), (int)H, (int)W, (uint32_t)ckey, (int32_t)bq, (int32_t)cq,
+                                    (int32_t)sq, (int32_t)hq, (int32_t)pq, (int)cluster, cur());
+  after();
+  TORCH_CHECK(G > 0, "augment_color: the cluster launch failed");
+  return G;
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -921,4 +958,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("zq"), py::arg("txq"), py::arg("tyq"), py::arg("mode"));
   m.def("augment_mix_warp", &augment_mix_warp, py::arg("x"), py::arg("out"), py::arg("params"), py::arg("mix"),
         py::arg("mode"), py::arg("fill_mode"), py::arg("fill_value"));
+  m.def("augment_color", &augment_color, py::arg("src"), py::arg("dst"), py::arg("step"), py::arg("H"), py::arg("W"),
+        py::arg("ckey"), py::arg("bq"), py::arg("cq"), py::arg("sq"), py::arg("hq"), py::arg("pq"),
+        py::arg("cluster") = 0);
 }

@@ -32,8 +32,8 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
     Keras's 154 ``base_model.layers``.  ``None`` (default) keeps the base frozen, or fully trainable with
     training-mode BatchNorm when ``freeze_base=False``; the two options cannot be combined.
 
-    ``augmentation`` (`Augmentation`): random flip / rotation / zoom / translation, and MixUp or CutMix, of every
-    training batch (Keras's augmentation layers in front of the model), on the device for the native engines;
+    ``augmentation`` (`Augmentation`): random flip / rotation / zoom / translation, MixUp or CutMix, and brightness /
+    contrast / saturation / hue / grayscale of every training batch (Keras's augmentation layers in front of the model), on the device for the native engines;
     ``evaluate`` / ``predict`` never augment.  ``None`` (default) leaves every path unchanged.  Not available for ``arch='resnet50_torch'``.
 
     ``batchnorm`` (MobileNetV2 with ``fine_tune_at`` only): ``"inference"`` (default) as above, or ``"training"`` - the

@@ -1,9 +1,9 @@
 """Random data augmentation in the training step: flip, rotation, zoom and translation (Keras ``RandomFlip``,
 ``RandomRotation``, ``RandomZoom``, ``RandomTranslation``), active in training only, as Keras preprocessing layers are.
 
-The native engines run it on the device inside the step's CUDA graph (csrc/augment.cu, two launches ahead of the stem).
-This module holds the configuration, the host-built rotation table, and the **reference implementation** - vectorised
-torch integer ops on any device - which reproduces both kernels bit for bit.  It is the training path of the torch
+The native engines run it on the device inside the step's CUDA graph (csrc/augment.cu, two launches ahead of the stem,
+and a third with color).  This module holds the configuration, the host-built rotation table, and the **reference
+implementation** - vectorised torch integer ops on any device - which reproduces every kernel bit for bit.  It is the training path of the torch
 modules (`FrozenBaseClassifier` on the module backend) and the oracle of the GPU tests.
 
 Differences from Keras, on purpose:
@@ -24,6 +24,19 @@ Draw 5 indexes a host-built table of 4096 Beta quantiles, draws 6 and 7 place th
 - The partners are a rotation of the batch (every image gets a different partner, and the rotation changes every step),
   not a uniformly random permutation; each data-parallel rank mixes within its own batch.
 - lambda is one of 4096 quantiles of Beta(alpha, alpha), and MixUp weights are quantised to 1/256.
+
+Color augmentation (``brightness``, ``contrast``, ``saturation``, ``hue``, ``grayscale``: Keras's ``RandomBrightness``,
+``RandomContrast``, ``RandomSaturation``, ``RandomHue`` and ``RandomGrayscale``) runs after the warp and the mixing, in
+that order, as one more launch (csrc/augment.cu augment_color).  Its draws come from their own key,
+``color_key(key) = hash_u32(key, 0x436F6C72, 0)``: draw ``k`` of image ``n`` is ``hash_u32(color_key(key), t, 8 n + k)``,
+so turning color on leaves every geometric and mix draw as it was.  The chain is integer arithmetic on Q8 values
+``v = 256 p``, rounded once at the end (see `color_reference`).  Differences from Keras:
+- Color is applied after the geometric warp and after mixing, and a mixed image takes image n's color draws; Keras
+  would color each source image before mixing them.
+- ``saturation`` s and ``hue`` h apply Keras 3's ``RandomSaturation`` / ``RandomHue`` HSV transforms but are
+  parametrised like ``contrast``: the saturation factor is uniform in [1 - s, 1 + s] (the result capped at 1), the hue
+  shift uniform in [-h, h] of a full turn.  Only scalar factors are accepted, not Keras's ``(lower, upper)`` tuples.
+- Factors are drawn on a 2^-16 grid (the brightness delta on a 1/256-level grid) and the chain runs in Q8 fixed point.
 """
 from __future__ import annotations
 
@@ -44,6 +57,11 @@ PARAM_FIELDS = 8       # a00 a01 b0 a10 a11 b1 flags 0
 MIX_FIELDS = 8         # partner, MixUp weight w, CutMix box x0 y0 x1 y1, mu = num / den
 MIX_NONE, MIX_UP, CUT_MIX = 0, 1, 2   # csrc/ops_api.h AugMix
 MAX_MIX_ALPHA = 100.0
+COLOR_FIELDS = (("brightness", 1.0), ("contrast", 1.0), ("saturation", 1.0), ("hue", 0.5), ("grayscale", 1.0))
+COLOR_SALT = 0x436F6C72        # color_key(key) = hash_u32(key, COLOR_SALT, 0)
+Q8_MAX = 255 * 256             # a channel's Q8 ceiling
+GRAY_WEIGHTS = (0.2989, 0.5870, 0.1140)
+GRAY_Q16 = (19589, 38470, 7471)   # rint(65536 * GRAY_WEIGHTS), csrc/augment.cu kGrayR / kGrayG / kGrayB
 _M32 = 0xFFFFFFFF
 
 
@@ -55,7 +73,14 @@ class Augmentation:
     [-f, f] of W / H, 0 <= f <= 1;  ``fill_mode``: "reflect" (d c b a | a b c d | d c b a) or "constant" with the uint8
     ``fill_value``;  ``mixup`` / ``cutmix``: the alpha of Beta(alpha, alpha) for Keras's MixUp / CutMix, in [0, 100],
     0 = off, at most one of them non-zero.  Mixing needs a loss that takes soft targets: the engines' head and the
-    module backend form them from the integer labels (see `train.losses.CategoricalCrossentropy`)."""
+    module backend form them from the integer labels (see `train.losses.CategoricalCrossentropy`).
+
+    Color, applied after the warp and the mixing in this order, each 0 = off:  ``brightness`` b in [0, 1]: add a
+    delta uniform in [-b, b] x 255 levels, then clip to [0, 255];  ``contrast`` c in [0, 1]: (x - mean) f + mean per
+    channel, f uniform in [1 - c, 1 + c], mean over the image, then clip;  ``saturation`` s in [0, 1]: HSV saturation
+    times a factor uniform in [1 - s, 1 + s], capped at 1;  ``hue`` h in [0, 0.5]: HSV hue rotated by a fraction of
+    a turn uniform in [-h, h];  ``grayscale`` p in [0, 1]: with probability p every channel becomes
+    0.2989 R + 0.5870 G + 0.1140 B."""
 
     flip: Optional[str] = None
     rotation: float = 0.0
@@ -65,6 +90,11 @@ class Augmentation:
     fill_value: int = 0
     mixup: float = 0.0
     cutmix: float = 0.0
+    brightness: float = 0.0
+    contrast: float = 0.0
+    saturation: float = 0.0
+    hue: float = 0.0
+    grayscale: float = 0.0
 
     def __post_init__(self):
         if self.flip not in FLIP_MODES:
@@ -88,6 +118,14 @@ class Augmentation:
             object.__setattr__(self, name, float(v))
         if self.mixup > 0 and self.cutmix > 0:
             raise ValueError(f"mixup and cutmix cannot both be on (got mixup={self.mixup}, cutmix={self.cutmix})")
+        for name, hi in COLOR_FIELDS:
+            v = getattr(self, name)
+            if isinstance(v, (tuple, list)):
+                raise ValueError(f"{name} takes one number in [0, {hi:g}]; Keras's (lower, upper) form is not "
+                                 f"supported, got {v!r}")
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or not 0.0 <= v <= hi:
+                raise ValueError(f"{name} must be a number in [0, {hi:g}], got {v!r}")
+            object.__setattr__(self, name, float(v))
 
     def to_dict(self) -> dict:
         return asdict(self)
@@ -104,6 +142,23 @@ class Augmentation:
     def mix_mode(self) -> int:
         """MIX_NONE, MIX_UP or CUT_MIX (csrc/ops_api.h AugMix)."""
         return MIX_UP if self.mixup > 0 else CUT_MIX if self.cutmix > 0 else MIX_NONE
+
+    @property
+    def color_on(self) -> bool:
+        return any(getattr(self, name) > 0 for name, _ in COLOR_FIELDS)
+
+    @property
+    def warp_on(self) -> bool:
+        """Whether the params + warp launches have work: a geometric or mix field is set, or nothing at all is (the
+        identity configuration keeps its two launches)."""
+        geometric = self.flip is not None or self.rotation > 0 or self.zoom > 0 or self.translation > 0
+        return geometric or self.mix_mode != MIX_NONE or not self.color_on
+
+    def color_quantised(self) -> Tuple[int, int, int, int, int]:
+        """The half-ranges augment_color takes: brightness in Q8 levels, contrast and saturation in Q16, hue in Q16
+        sixths of a turn, the grayscale probability in Q16."""
+        return (int(round(self.brightness * Q8_MAX)), int(round(self.contrast * 65536)),
+                int(round(self.saturation * 65536)), int(round(self.hue * 6 * 65536)), int(round(self.grayscale * 65536)))
 
     def lambda_table(self) -> torch.Tensor:
         """int32 [4096, 2]: rint(65536 lambda_i) and rint(65536 sqrt(1 - lambda_i)) for the Beta(alpha, alpha)
@@ -328,19 +383,120 @@ def mix_warp_reference(x_u8: torch.Tensor, params: torch.Tensor, mix: torch.Tens
     return torch.where(box.unsqueeze(-1), other, own).to(torch.uint8)
 
 
+def color_key(key: int) -> int:
+    """The uint32 key of the color draws: a fixed function of `augment_key`'s key, so they are independent of the
+    geometric and mix draws and leave them unchanged."""
+    return int(hash_u32(int(key) & _M32, COLOR_SALT, 0))
+
+
+def color_draws_reference(aug: Augmentation, N: int, key: int, step: int, device=None) -> torch.Tensor:
+    """int64 [N, 5]: the color draws augment_color makes for every image - brightness delta (Q8 levels), contrast
+    factor f and saturation factor S (Q16), hue shift (Q16 sixths of a turn), grayscale flag.  A stage that is off
+    holds its identity value (0, 65536, 65536, 0, 0)."""
+    dev = torch.device(device) if device is not None else torch.device("cpu")
+    bq, cq, sq, hq, pq = aug.color_quantised()
+    c = torch.arange(N, device=dev, dtype=torch.int64) * 8
+    t = int(step) & 0x7FFFFFFF
+    ck = color_key(key)
+    u = [hash_u32(ck, t, c + k) >> 16 for k in range(5)]
+
+    def uniform(v, q):   # uniform in [-q, q) on a 2^-16 grid
+        return -q + ((2 * q * v) >> 16)
+
+    return torch.stack([uniform(u[0], bq), 65536 + uniform(u[1], cq), 65536 + uniform(u[2], sq), uniform(u[3], hq),
+                        (u[4] < pq).to(torch.int64)], 1)
+
+
+def _saturate(r, g, b, S):
+    """v' = mx - (mx - v) k with k = min(S, mx / dl) in Q16: the max (HSV value) is kept and the saturation dl / mx
+    scaled by S, capped at 1.  k = S whenever S <= 1, since mx >= dl.  A pixel with dl = 0 is unchanged."""
+    mx = torch.maximum(r, torch.maximum(g, b))
+    dl = mx - torch.minimum(r, torch.minimum(g, b))
+    k = torch.where(S <= 65536, S, torch.minimum(S, (mx << 16) // dl.clamp(min=1)))
+    return tuple(mx - (((mx - v) * k + 32768) >> 16) for v in (r, g, b))
+
+
+def _rotate_hue(r, g, b, dh):
+    """The hue position P in Q16 sixths of a turn (the max channel taken in the order R, G, B; the fraction rounded
+    half up), rotated by dh modulo a turn; the pixel is rebuilt from (sector P >> 16, fraction P & 65535) with its max
+    and min kept.  A pixel with dl = 0 comes back unchanged (every candidate value equals it)."""
+    mx = torch.maximum(r, torch.maximum(g, b))
+    mn = torch.minimum(r, torch.minimum(g, b))
+    dl = mx - mn
+    dls = dl.clamp(min=1)
+
+    def frac(a):
+        return (a * 65536 + (dls >> 1)) // dls
+
+    turn = 6 * 65536
+    P = torch.where(r == mx, torch.where(g >= b, frac(g - b), turn - frac(b - g)),
+                    torch.where(g == mx, 2 * 65536 + torch.where(b >= r, frac(b - r), -frac(r - b)),
+                                4 * 65536 + torch.where(r >= g, frac(r - g), -frac(g - r))))
+    P = (P + dh + 2 * turn) % turn
+    part = ((P & 65535) * dl + 32768) >> 16
+    rise, fall = mn + part, mx - part
+    sec = (P >> 16).unsqueeze(-1)
+
+    def pick(*vals):   # the value of sector 0 .. 5
+        return torch.stack(torch.broadcast_tensors(*vals), -1).gather(-1, sec).squeeze(-1)
+
+    return (pick(mx, fall, mn, mn, rise, mx), pick(rise, mx, mx, fall, mn, mn), pick(mn, mn, rise, mx, mx, fall))
+
+
+def color_apply_reference(x_u8: torch.Tensor, draws: torch.Tensor, stages) -> torch.Tensor:
+    """augment_color's chain on the uint8 [N, H, W, 3] batch with the per-image ``draws`` of `color_draws_reference`;
+    ``stages``: five booleans (brightness, contrast, saturation, hue, grayscale), False skipping the stage.  Q8 values
+    v = 256 p in int64; clamped to [0, 255 * 256] after brightness and after contrast; contrast uses the per-channel
+    mean round(sum v / (H W)) of the post-brightness image (an exact integer sum); one rounding (v + 128) >> 8 at the
+    end."""
+    N, H, W, _ = x_u8.shape
+    d = draws.to(x_u8.device, torch.int64)
+    bright, contrast, saturation, hue, gray = (bool(s) for s in stages)
+    v = x_u8.to(torch.int64) << 8
+    if bright:
+        v = (v + d[:, 0].view(N, 1, 1, 1)).clamp(0, Q8_MAX)
+    if contrast:
+        mean = (v.sum((1, 2), keepdim=True) + (H * W) // 2) // (H * W)
+        v = (mean + (((v - mean) * d[:, 1].view(N, 1, 1, 1) + 32768) >> 16)).clamp(0, Q8_MAX)
+    r, g, b = v.unbind(-1)
+    if saturation:
+        r, g, b = _saturate(r, g, b, d[:, 2].view(N, 1, 1))
+    if hue:
+        r, g, b = _rotate_hue(r, g, b, d[:, 3].view(N, 1, 1))
+    if gray:
+        y = (GRAY_Q16[0] * r + GRAY_Q16[1] * g + GRAY_Q16[2] * b + 32768) >> 16
+        on = d[:, 4].view(N, 1, 1) != 0
+        r, g, b = (torch.where(on, y, c) for c in (r, g, b))
+    return ((torch.stack([r, g, b], -1) + 128) >> 8).to(torch.uint8)
+
+
+def color_reference(aug: Augmentation, x_u8: torch.Tensor, key: int, step: int) -> torch.Tensor:
+    """augment_color: the color augmentation of the uint8 [N, H, W, 3] batch at optimizer step ``step``, ``key`` being
+    `augment_key`'s (the color key is derived from it)."""
+    draws = color_draws_reference(aug, x_u8.shape[0], key, step, device=x_u8.device)
+    return color_apply_reference(x_u8, draws, [q > 0 for q in aug.color_quantised()])
+
+
 def augment_batch_reference(aug: Augmentation, x_u8: torch.Tensor, key: int, step: int):
     """What the engines' training step feeds its stem and its head: the warp of the uint8 NHWC batch at optimizer step
-    ``step``, mixed with the partners' warps when MixUp or CutMix is on, and the mix rows (None without mixing)."""
+    ``step``, mixed with the partners' warps when MixUp or CutMix is on, then colored when a color field is on, and
+    the mix rows (None without mixing)."""
     if x_u8.dtype != torch.uint8 or x_u8.dim() != 4 or x_u8.shape[3] != 3:
         raise ValueError(f"augmentation needs a uint8 [N, H, W, 3] batch, got {tuple(x_u8.shape)} {x_u8.dtype}")
     N, H, W, _ = x_u8.shape
     if max(H, W) > MAX_SIDE:
         raise ValueError(f"augmentation: image sides must be at most {MAX_SIDE}")
-    params = params_reference(aug, N, H, W, key, step, device=x_u8.device)
-    if aug.mix_mode == MIX_NONE:
-        return warp_reference(x_u8, params, aug.fill_mode, aug.fill_value), None
-    mix = mix_params_reference(aug, N, H, W, key, step, device=x_u8.device)
-    return mix_warp_reference(x_u8, params, mix, aug.mix_mode, aug.fill_mode, aug.fill_value), mix
+    out, mix = x_u8, None
+    if aug.warp_on:
+        params = params_reference(aug, N, H, W, key, step, device=x_u8.device)
+        if aug.mix_mode == MIX_NONE:
+            out = warp_reference(x_u8, params, aug.fill_mode, aug.fill_value)
+        else:
+            mix = mix_params_reference(aug, N, H, W, key, step, device=x_u8.device)
+            out = mix_warp_reference(x_u8, params, mix, aug.mix_mode, aug.fill_mode, aug.fill_value)
+    if aug.color_on:
+        out = color_reference(aug, out, key, step)
+    return out, mix
 
 
 def augment_reference(aug: Augmentation, x_u8: torch.Tensor, key: int, step: int) -> torch.Tensor:
@@ -404,7 +560,8 @@ class DeviceAugmenter:
     warp of ``x`` into ``out``.  The engine owns the buffers; the host writes the step word with `set_step` (a pinned
     ring slot and an async copy, as the optimizer hyper-parameters are written), never as a kernel argument.  With
     MixUp or CutMix the same two launches also write the mix rows ``mix`` (the soft-target head reads them) and mix
-    every image with its partner; without, ``mix`` is None."""
+    every image with its partner; without, ``mix`` is None.  With a color field on, augment_color follows in place on
+    ``out``; when color is all there is, it is the only launch and reads ``x``."""
 
     def __init__(self, aug: Augmentation, x: torch.Tensor, seed: int, rank: int = 0):
         from .. import ops
@@ -427,6 +584,8 @@ class DeviceAugmenter:
         if aug.mix_mode != MIX_NONE:
             self.mix = torch.zeros(N, MIX_FIELDS, device=x.device, dtype=torch.int32)
             self.lam_table = aug.lambda_table().to(x.device)
+        self.color = aug.color_quantised() if aug.color_on else None
+        self.ckey = color_key(self.key)
 
     def set_step(self, t: int) -> None:
         """Host -> device write of the step word (outside any CUDA graph; the graph reads it on replay)."""
@@ -452,6 +611,19 @@ class DeviceAugmenter:
             return
         self._e.augment_warp(self.x, self.out, self.params, self.aug.fill_mode, self.aug.fill_value)
 
+    def run_color(self, cluster: int = 0) -> int:
+        """augment_color: ``out`` colored in place after the warp, or from ``x`` when there is no warp.  ``cluster``
+        forces the CTAs per image (tests and benchmarks; the bytes are the same for every value).  Returns the cluster
+        size launched."""
+        if self.color is None:
+            raise ValueError("run_color: no color field is on")
+        _, H, W, _ = self.x.shape
+        src = self.out if self.aug.warp_on else self.x
+        return self._e.augment_color(src, self.out, self.step, H, W, self.ckey, *self.color, cluster)
+
     def run(self) -> None:
-        self.run_params()
-        self.run_warp()
+        if self.aug.warp_on:
+            self.run_params()
+            self.run_warp()
+        if self.color is not None:
+            self.run_color()
