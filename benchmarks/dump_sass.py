@@ -24,7 +24,7 @@ COUNT = [("HGMMA", r"\bHGMMA\b"), ("UTMALDG", r"\bUTMALDG"), ("UTMASTG", r"\bUTM
 SELECT = ["conv_igemm_kernel<64, 1, true, true>", "conv_igemm_kernel<64, 2, true, true>", "conv_igemm_kernel<128, 1, false, false>",
           "conv_igemm_kernel<128, 2, false, false>", "conv_igemm_kernel<128, 3, false, false>", "conv_igemm_kernel<128, 4, false, false>",
           "allreduce_twoshot_nvls_kernel<(b200::CommDtype)0, 8>", "broadcast_kernel<(b200::CommDtype)0>", "stem_pool_bn_bwd_kernel<0>",
-          "softmax_ce_head_kernel", "softmax_ce_soft_head_kernel", "augment_mix_params_kernel", "augment_mix_warp_kernel<1>",
+          "softmax_ce_head_kernel", "softmax_ce_soft_head_kernel", "softmax_kd_head_kernel", "augment_mix_params_kernel", "augment_mix_warp_kernel<1>",
           "augment_mix_warp_kernel<2>", "augment_color_kernel", "dwconv3x3_kernel<1>", "dwconv3x3_tiled_kernel<1, 4>", "resize_triangle_batched_kernel", "mbv2_stem_kernel", "weight_prep_batched_kernel", "conv_wgrad_kernel", "stem_fwd_kernel", "stem_wgrad_kernel",
           "allreduce_twoshot_nvls_kernel<(b200::CommDtype)0", "allreduce_sgd_nvls_kernel", "allreduce_twoshot_p2p_kernel<(b200::CommDtype)0, 2>",
           "bn_apply_kernel<true, 1, false, 1>", "col_reduce_kernel<4>", "bn_bwd_apply_kernel<true, false, 1>", "update_kernel<b200::SgdRule<false> >",

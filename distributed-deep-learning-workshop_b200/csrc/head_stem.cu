@@ -181,6 +181,121 @@ void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const
                                                          loss_rows, stats, B, K, grad_scale);
 }
 
+// softmax_ce_soft_head plus knowledge distillation from a teacher's logits t (bf16 tlogits16 [B, tld] + tbias), at
+// weight alpha and temperature T; s = the student's logits (bias included):
+//   loss    = alpha * ce + (1 - alpha) * kd,   ce = softmax_ce_soft_head's loss,   kd = T^2 KL(r || q)
+//   KL      = sum_k r_k (log r_k - log q_k),   r = softmax(t / T), q = softmax(s / T)   (the two log-softmaxes, no clipping)
+//   dlogits = (alpha (p_k - target_k) + (1 - alpha) T (q_k - r_k)) * grad_scale
+//   stats   = [sum loss, correct, sum ce, sum kd]
+// The student part is softmax_ce_soft_head's code, then scaled by alpha and added to the distillation part scaled by
+// 1 - alpha with correctly rounded, uncontracted operations: at alpha = 1 that is a product by 1 plus a product by 0, so
+// loss, dlogits and loss_rows are bit for bit softmax_ce_soft_head's (and softmax_ce_head's at eps = 0 without mix
+// rows).  The teacher's row is only read: its max, then exp((t - tmax) / T) twice.
+__global__ void softmax_kd_head_kernel(const __nv_bfloat16* __restrict__ logits16, int ld,
+                                       const float* __restrict__ bias, const __nv_bfloat16* __restrict__ tlogits16,
+                                       int tld, const float* __restrict__ tbias, const int64_t* __restrict__ labels,
+                                       const int4* __restrict__ mix, float eps, float alpha, float T,
+                                       float* __restrict__ logits32, __nv_bfloat16* __restrict__ dlogits16,
+                                       float* __restrict__ loss_rows, float* __restrict__ stats, int B, int K,
+                                       float grad_scale) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (warp >= B) return;
+  const __nv_bfloat16* row = logits16 + (int64_t)warp * ld;
+  const __nv_bfloat16* trow = tlogits16 + (int64_t)warp * tld;
+  const int label = (int)labels[warp];
+  int plabel = label, target = label;
+  float mu = 0.f;
+  if (mix != nullptr) {
+    const int4 m0 = mix[2 * warp], m1 = mix[2 * warp + 1];
+    plabel = (int)labels[(unsigned)m0.x < (unsigned)B ? m0.x : warp];
+    mu = __fdiv_rn((float)m1.z, (float)m1.w);
+    if (plabel != label) {
+      const int64_t twice = 2 * (int64_t)m1.z;
+      target = twice < m1.w ? label : twice > m1.w ? plabel : min(label, plabel);
+    }
+  }
+  const float lam = 1.f - mu, keep = 1.f - eps, epsk = __fdiv_rn(eps, (float)K);
+  const float beta = 1.f - alpha, invT = __fdiv_rn(1.f, T);
+  float mx = -3.0e38f, tmx = -3.0e38f;
+  int amax = 0;
+  for (int k = lane; k < K; k += 32) {
+    const float v = __bfloat162float(row[k]) + bias[k];
+    if (logits32 != nullptr) logits32[(int64_t)warp * K + k] = v;
+    if (v > mx) { mx = v; amax = k; }
+    tmx = fmaxf(tmx, __bfloat162float(trow[k]) + tbias[k]);
+  }
+  for (int o = 16; o; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+    const int oa = __shfl_xor_sync(0xffffffffu, amax, o);
+    if (om > mx || (om == mx && oa < amax)) { mx = om; amax = oa; }
+    tmx = fmaxf(tmx, __shfl_xor_sync(0xffffffffu, tmx, o));
+  }
+  // the max of s / T and t / T is max / T (T > 0): (v - max) / T <= 0 in every exponent
+  float se = 0.f, sd = 0.f, seT = 0.f, teT = 0.f;
+  for (int k = lane; k < K; k += 32) {
+    const float v = __bfloat162float(row[k]) + bias[k];
+    se += __expf(v - mx);
+    sd += mx - v;
+    seT += __expf((v - mx) * invT);
+    teT += __expf((__bfloat162float(trow[k]) + tbias[k] - tmx) * invT);
+  }
+  for (int o = 16; o; o >>= 1) {
+    se += __shfl_xor_sync(0xffffffffu, se, o);
+    sd += __shfl_xor_sync(0xffffffffu, sd, o);
+    seT += __shfl_xor_sync(0xffffffffu, seT, o);
+    teT += __shfl_xor_sync(0xffffffffu, teT, o);
+  }
+  const float lse = mx + __logf(se);
+  const float inv = 1.f / se;
+  const float lseT = __logf(seT), lteT = __logf(teT);   // log-normalisers of (s - max) / T and (t - tmax) / T
+  const float invS = 1.f / seT, invTe = 1.f / teT;
+  float kl = 0.f;
+  __nv_bfloat16* drow = dlogits16 != nullptr ? dlogits16 + (int64_t)warp * ld : nullptr;
+  for (int k = lane; k < (drow != nullptr ? ld : K); k += 32) {
+    float d = 0.f;
+    if (k < K) {
+      const float v = __bfloat162float(row[k]) + bias[k];
+      const float zs = (v - mx) * invT;
+      const float zt = (__bfloat162float(trow[k]) + tbias[k] - tmx) * invT;
+      const float rk = __expf(zt) * invTe;
+      kl += rk * ((zt - lteT) - (zs - lseT));
+      if (drow != nullptr) {
+        const float pk = __expf(v - mx) * inv;
+        const float tk = keep * ((k == label ? lam : 0.f) + (k == plabel ? mu : 0.f)) + epsk;
+        const float qk = __expf(zs) * invS;
+        const float ds = (pk - tk) * grad_scale;   // softmax_ce_soft_head's dlogit
+        d = __fadd_rn(__fmul_rn(alpha, ds), __fmul_rn(beta, T * (qk - rk) * grad_scale));
+      }
+    }
+    if (drow != nullptr) drow[k] = __float2bfloat16(d);
+  }
+  for (int o = 16; o; o >>= 1) kl += __shfl_xor_sync(0xffffffffu, kl, o);
+  if (lane == 0) {
+    const float ly = __bfloat162float(row[label]) + bias[label];
+    const float lp = __bfloat162float(row[plabel]) + bias[plabel];
+    const float ce = keep * (lam * (lse - ly) + mu * (lse - lp)) + epsk * (sd + (float)K * (lse - mx));
+    const float kd = T * T * kl;
+    const float l = __fadd_rn(__fmul_rn(alpha, ce), __fmul_rn(beta, kd));   // no contraction: alpha = 1 gives ce
+    if (loss_rows != nullptr) loss_rows[warp] = l;
+    atomicAdd(stats, l);
+    atomicAdd(stats + 1, amax == target ? 1.f : 0.f);
+    atomicAdd(stats + 2, ce);
+    atomicAdd(stats + 3, kd);
+  }
+}
+void softmax_kd_head(const void* logits16, int ld, const float* bias, const void* tlogits16, int tld,
+                     const float* tbias, const int64_t* labels, const int32_t* mix, float eps, float alpha, float T,
+                     float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale,
+                     cudaStream_t s) {
+  const int threads = 128;
+  const int blocks = (B * 32 + threads - 1) / threads;
+  softmax_kd_head_kernel<<<blocks, threads, 0, s>>>((const __nv_bfloat16*)logits16, ld, bias,
+                                                    (const __nv_bfloat16*)tlogits16, tld, tbias, labels,
+                                                    (const int4*)mix, eps, alpha, T, logits32,
+                                                    (__nv_bfloat16*)dlogits16, loss_rows, stats, B, K, grad_scale);
+}
+
 // dbias[k] = sum_b dlogits16[b, k]   (thread per column: coalesced across k for every row)
 __global__ void fc_bias_grad_kernel(const __nv_bfloat16* __restrict__ dl, int ld, float* __restrict__ dbias, int B, int K) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;

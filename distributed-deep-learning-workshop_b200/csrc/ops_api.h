@@ -182,5 +182,11 @@ int augment_color(const uint8_t* src, uint8_t* dst, const int32_t* step, int N, 
 void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const int64_t* labels, const int32_t* mix,
                           float eps, float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K,
                           float grad_scale, cudaStream_t s);
+// softmax_ce_soft_head's loss at weight alpha plus (1 - alpha) T^2 KL(softmax(t / T) || softmax(s / T)), t = the
+// teacher's bf16 logits [B, tld] + tbias; stats = [sum loss, correct, sum soft-target loss, sum T^2 KL]
+void softmax_kd_head(const void* logits16, int ld, const float* bias, const void* tlogits16, int tld,
+                     const float* tbias, const int64_t* labels, const int32_t* mix, float eps, float alpha, float T,
+                     float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale,
+                     cudaStream_t s);
 
 }  // namespace b200

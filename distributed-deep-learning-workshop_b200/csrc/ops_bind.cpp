@@ -351,6 +351,63 @@ void softmax_ce_soft_head(Tensor logits16, Tensor bias, Tensor labels, OptT mix,
                              K, (float)grad_scale, cur());
   after();
 }
+// softmax_ce_soft_head plus distillation from the teacher's bf16 logits [B, tld] + tbias (tld >= K = bias.numel()) at
+// weight 1 - alpha and temperature T; stats: [sum loss, correct, sum student loss, sum distillation loss]
+void softmax_kd_head(Tensor logits16, Tensor bias, Tensor tlogits16, Tensor tbias, Tensor labels, OptT mix, double eps,
+                     double alpha, double temperature, OptT logits32, OptT dlogits16, OptT loss_rows, Tensor stats,
+                     double grad_scale) {
+  chk(logits16, at::kBFloat16, "logits16");
+  chk(bias, at::kFloat, "bias");
+  chk(tlogits16, at::kBFloat16, "tlogits16");
+  chk(tbias, at::kFloat, "tbias");
+  chk(labels, at::kLong, "labels");
+  chk(stats, at::kFloat, "stats");
+  TORCH_CHECK(logits16.dim() == 2 && logits16.size(0) >= 1 && bias.numel() >= 1 && bias.numel() <= logits16.size(1) &&
+                  labels.numel() == logits16.size(0),
+              "logits16 must be bf16 [B, ld] with ld >= K = bias.numel() and B = labels.numel() >= 1");
+  TORCH_CHECK(tlogits16.dim() == 2 && tlogits16.size(0) == logits16.size(0) && tbias.numel() == bias.numel() &&
+                  tlogits16.size(1) >= bias.numel(),
+              "tlogits16 must be bf16 [B, tld] with tld >= K and tbias must hold K values");
+  TORCH_CHECK(stats.numel() >= 4, "stats must hold [sum loss, correct, sum student loss, sum distillation loss]");
+  TORCH_CHECK(eps >= 0.0 && eps <= 1.0, "label smoothing must be in [0, 1]");
+  TORCH_CHECK(alpha >= 0.0 && alpha <= 1.0, "alpha must be in [0, 1]");
+  TORCH_CHECK(temperature > 0.0 && temperature < 1e30, "temperature must be finite and > 0");
+  const int B = (int)logits16.size(0), ld = (int)logits16.size(1), tld = (int)tlogits16.size(1), K = (int)bias.numel();
+  for (const Tensor* t : {&bias, &tlogits16, &tbias, &labels, &stats})
+    TORCH_CHECK(t->device() == logits16.device(), "bias, the teacher's tensors, labels and stats must be on the device "
+                "of logits16");
+  if (mix.has_value()) {
+    chk(*mix, at::kInt, "mix");
+    TORCH_CHECK(mix->dim() == 2 && mix->size(0) == B && mix->size(1) == b200::kAugMixFields,
+                "mix must be int32 [B, 8] for the batch's B rows");
+    TORCH_CHECK(mix->device() == logits16.device(), "mix must be on the device of logits16");
+    aligned(*mix, 16, "mix");
+  }
+  if (logits32.has_value()) {
+    chk(*logits32, at::kFloat, "logits32");
+    TORCH_CHECK(logits32->numel() == (int64_t)B * K, "logits32 must hold B x K values");
+  }
+  if (dlogits16.has_value()) {
+    chk(*dlogits16, at::kBFloat16, "dlogits16");
+    TORCH_CHECK(dlogits16->numel() == logits16.numel(), "dlogits16 must have the shape of logits16");
+    TORCH_CHECK(dlogits16->data_ptr() != logits16.data_ptr() && dlogits16->data_ptr() != tlogits16.data_ptr(),
+                "dlogits16 cannot overwrite logits16 or tlogits16");
+  }
+  if (loss_rows.has_value()) {
+    chk(*loss_rows, at::kFloat, "loss_rows");
+    TORCH_CHECK(loss_rows->numel() == B, "loss_rows must hold B values");
+  }
+  for (const OptT* t : {&logits32, &dlogits16, &loss_rows})
+    if (t->has_value()) TORCH_CHECK((*t)->device() == logits16.device(), "outputs must be on the device of logits16");
+  b200::softmax_kd_head(logits16.data_ptr(), ld, bias.data_ptr<float>(), tlogits16.data_ptr(), tld,
+                        tbias.data_ptr<float>(), labels.data_ptr<int64_t>(),
+                        mix.has_value() ? mix->data_ptr<int32_t>() : nullptr, (float)eps, (float)alpha,
+                        (float)temperature, logits32.has_value() ? logits32->data_ptr<float>() : nullptr,
+                        dlogits16.has_value() ? dlogits16->data_ptr() : nullptr,
+                        loss_rows.has_value() ? loss_rows->data_ptr<float>() : nullptr, stats.data_ptr<float>(), B, K,
+                        (float)grad_scale, cur());
+  after();
+}
 void fc_bias_grad(Tensor dlogits16, Tensor dbias) {
   chk(dlogits16, at::kBFloat16, "dlogits16");
   chk(dbias, at::kFloat, "dbias");
@@ -909,6 +966,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("stats"), py::arg("grad_scale") = 1.0);
   m.def("softmax_ce_soft_head", &softmax_ce_soft_head, py::arg("logits16"), py::arg("bias"), py::arg("labels"),
         py::arg("mix") = c10::nullopt, py::arg("label_smoothing") = 0.0, py::arg("logits32") = c10::nullopt,
+        py::arg("dlogits16") = c10::nullopt, py::arg("loss_rows") = c10::nullopt, py::arg("stats"),
+        py::arg("grad_scale") = 1.0);
+  m.def("softmax_kd_head", &softmax_kd_head, py::arg("logits16"), py::arg("bias"), py::arg("tlogits16"),
+        py::arg("tbias"), py::arg("labels"), py::arg("mix") = c10::nullopt, py::arg("label_smoothing") = 0.0,
+        py::arg("alpha") = 0.1, py::arg("temperature") = 3.0, py::arg("logits32") = c10::nullopt,
         py::arg("dlogits16") = c10::nullopt, py::arg("loss_rows") = c10::nullopt, py::arg("stats"),
         py::arg("grad_scale") = 1.0);
   m.def("fc_bias_grad", &fc_bias_grad);

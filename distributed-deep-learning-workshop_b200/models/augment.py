@@ -555,6 +555,45 @@ def soft_head_reference(logits: torch.Tensor, labels: torch.Tensor, mix: Optiona
     return loss, d, correct
 
 
+def distillation_reference(logits: torch.Tensor, teacher_logits: torch.Tensor, labels: torch.Tensor,
+                           mix: Optional[torch.Tensor] = None, label_smoothing: float = 0.0, alpha: float = 0.1,
+                           temperature: float = 3.0):
+    """Per-row losses of `train.losses.Distillation` (softmax_kd_head), in the dtype of ``logits`` [B, K] (bias
+    included) and differentiable: (loss, student term, distillation term) with
+
+        student = sum_k target_k (lse(s) - s_k),   target = `soft_targets` (smoothed, mixed)
+        distill = T^2 KL(softmax(t / T) || softmax(s / T)),   from the two log-softmaxes (no clipping)
+        loss    = alpha student + (1 - alpha) distill
+
+    The module backend trains on it (fp32, autograd); in float64 it is the kernel's reference."""
+    s = logits
+    t = teacher_logits.to(s.dtype)
+    T = float(temperature)
+    tgt = soft_targets(labels, s.shape[1], mix, label_smoothing, s.dtype)
+    student = (tgt * (torch.logsumexp(s, 1, keepdim=True) - s)).sum(1)
+    lr = torch.log_softmax(t / T, 1)
+    lq = torch.log_softmax(s / T, 1)
+    distill = T * T * (lr.exp() * (lr - lq)).sum(1)
+    return alpha * student + (1 - alpha) * distill, student, distill
+
+
+def distillation_head_reference(logits: torch.Tensor, teacher_logits: torch.Tensor, labels: torch.Tensor,
+                                mix: Optional[torch.Tensor] = None, label_smoothing: float = 0.0, alpha: float = 0.1,
+                                temperature: float = 3.0, grad_scale: float = 1.0):
+    """float64 softmax_kd_head of fp32 ``logits`` / ``teacher_logits`` [B, K] (biases included): the per-row
+    (loss, student term, distillation term) of `distillation_reference`, dlogits
+    (alpha (softmax(s) - target) + (1 - alpha) T (softmax(s / T) - softmax(t / T))) * grad_scale, and the correct
+    count of `soft_head_reference`."""
+    z, zt = logits.double(), teacher_logits.double()
+    T = float(temperature)
+    loss, student, distill = distillation_reference(z, zt, labels, mix, label_smoothing, alpha, T)
+    tgt = soft_targets(labels, z.shape[1], mix, label_smoothing, torch.float64)
+    d = (alpha * (torch.softmax(z, 1) - tgt) + (1 - alpha) * T * (torch.softmax(z / T, 1) - torch.softmax(zt / T, 1)))
+    am = torch.from_numpy(np.argmax(logits.detach().cpu().numpy(), axis=1)).to(labels.device)
+    correct = int((am == target_argmax(labels, mix)).sum())
+    return loss, student, distill, d * grad_scale, correct
+
+
 class DeviceAugmenter:
     """The two kernel launches of one engine: per-image parameters into ``params`` from the device step word, then the
     warp of ``x`` into ``out``.  The engine owns the buffers; the host writes the step word with `set_step` (a pinned

@@ -44,7 +44,7 @@ import torch
 
 from .. import ops
 from ..ops import conv as C
-from .resnet_engine import ParamSpec, _align, _augmenter
+from .resnet_engine import ParamSpec, _align, _augmenter, _kd_head, _stats_len, set_distillation
 
 _CFG = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2), (6, 320, 1, 1)]
 
@@ -76,6 +76,8 @@ class MobileNetV2Engine:
         self._augmenter = None
         # Keras's label smoothing of the loss; the Trainer sets it from the compiled loss before capturing the steps
         self.label_smoothing = 0.0
+        self.distillation = None   # `train.losses.Distillation` with an engine teacher: set by `set_distillation`
+        self._teacher_in: Optional[torch.Tensor] = None   # a student's stem input this engine reads as a teacher
         if image_size % 32:
             raise ValueError("image_size must be a multiple of 32")
         check_fine_tune_at(fine_tune_at)
@@ -308,7 +310,7 @@ class MobileNetV2Engine:
         f32 = dict(device=dev, dtype=torch.float32)
         self.x_u8 = torch.zeros(N, S, S, 3, device=dev, dtype=torch.uint8)
         self.labels = torch.zeros(N, device=dev, dtype=torch.int64)
-        self.stats = torch.zeros(2, **f32)
+        self.stats = torch.zeros(_stats_len(self), **f32)
         self.logits = torch.zeros(N, self.num_classes, **f32)
         self.loss_rows = torch.zeros(N, **f32)
         self._plan: List[dict] = []
@@ -530,17 +532,30 @@ class MobileNetV2Engine:
                 self._build_backward()
             self._augmenter = _augmenter(self, self.x_u8)
             self._training_built = True
+            if self.distillation is not None:
+                self.distillation.teacher.bind_teacher_input(self._stem_input(True))
 
     # ------------------------------------------------------------------------------------------------ forward / backward
     def forward(self, training: bool = True) -> None:
-        e, N = self._e, self.batch
+        self.forward_logits(training)
+        self.forward_head(training)
+
+    def forward_logits(self, training: bool = True, teacher: bool = False) -> None:
+        """Augmentation (training), a distillation teacher's logits (training), features and the bf16 FC logits
+        ``logits16``.  ``teacher=True``: the inference forward of this engine as a distillation teacher, reading the
+        student's stem input bound by `bind_teacher_input` instead of ``x_u8``."""
+        e = self._e
         if training and self._augmenter is not None:
             self._augmenter.run()
+        if training and self.distillation is not None:
+            # the teacher reads this step's stem input in place, before the stem: its logits16 feed the head
+            self.distillation.teacher.forward_logits(False, teacher=True)
         for lay in self._plan:
             if training and lay["train"] and self._bn_train:
                 self._forward_bn_train(lay)
             elif lay["kind"] == "stem":
-                e.mbv2_stem(self._stem_input(training), lay["w"], lay["scale"], lay["shift"], lay["y"], 1.0 / 127.5, -1.0)
+                x = self._teacher_in if teacher else self._stem_input(training)
+                e.mbv2_stem(x, lay["w"], lay["scale"], lay["shift"], lay["y"], 1.0 / 127.5, -1.0)
             elif lay["kind"] == "dw":
                 e.dwconv3x3(lay["x"], lay["w"], lay["scale"], lay["shift"], lay["y"], lay["stride"])
             else:
@@ -549,10 +564,16 @@ class MobileNetV2Engine:
         self._drop_seed = self.seed * 1000003 + self._step_count
         e.gap_fwd(self.feat, self.pooled, drop, self._drop_seed)
         self._fc_fwd.run()
+
+    def forward_head(self, training: bool = True) -> None:
+        """+ bias, softmax cross-entropy, accuracy, bf16 dlogits in one kernel (see `ResNet50Engine.forward_head`)."""
+        e, N = self._e, self.batch
         e.zero_(self.stats)
         dl = self.dlogits16 if (training and self._training_built) else None
         mix = self._augmenter.mix if (training and self._augmenter is not None) else None
-        if mix is None and self.label_smoothing == 0:
+        if training and self.distillation is not None:
+            _kd_head(self, mix, dl)
+        elif mix is None and self.label_smoothing == 0:
             e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits, dl, self.loss_rows,
                               self.stats, 1.0 / N)
         else:   # soft targets: the partner's label at the mix row's weight, label smoothing
@@ -608,6 +629,17 @@ class MobileNetV2Engine:
         """Step word the next training forward's augmentation reads (the optimizer's step counter)."""
         if self._augmenter is not None:
             self._augmenter.set_step(t)
+
+    def set_distillation(self, distillation) -> None:
+        """Distil from ``distillation.teacher`` in the training steps captured from now on (see
+        `resnet_engine.set_distillation`)."""
+        set_distillation(self, distillation)
+
+    def bind_teacher_input(self, x_u8: torch.Tensor) -> None:
+        """Teach a student whose stem reads ``x_u8``: build for inference if not built (as `EngineEvalStep` does);
+        ``forward_logits(training=False, teacher=True)`` then reads that buffer in place of this engine's own."""
+        self._teacher_in = x_u8
+        self.build(training=self.grads is not None)
 
     def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None) -> None:
         self.x_u8.copy_(x_u8.view(self.x_u8.shape), non_blocking=True)

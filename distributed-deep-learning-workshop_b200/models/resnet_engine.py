@@ -75,6 +75,33 @@ def _augmenter(engine, x_u8: torch.Tensor):
     return DeviceAugmenter(engine.augmentation, x_u8, engine.seed, _core.rank())
 
 
+def _stats_len(engine) -> int:
+    return 2 if engine.distillation is None else 4
+
+
+def set_distillation(student, distillation) -> None:
+    """Make ``student`` (either native engine) distil from ``distillation.teacher`` (a `train.losses.Distillation`
+    whose teacher is a native engine; None: plain training) in the training steps captured from now on.  The teacher
+    is bound to the student's stem input (built for inference on first use) and ``stats`` grows to four floats: [sum
+    loss, correct, sum student loss, sum distillation loss]."""
+    if distillation is not None:
+        distillation.check_student(student)
+    student.distillation = distillation
+    if distillation is not None and student._built and student._training_built:
+        distillation.teacher.bind_teacher_input(student._stem_input(True))   # else at the student's training build
+    if student._built and student.stats.numel() != _stats_len(student):
+        student.stats = torch.zeros(_stats_len(student), device=student.device, dtype=torch.float32)
+
+
+def _kd_head(student, mix, dlogits16) -> None:
+    """softmax_kd_head of a distilling student's logits16 against its teacher's (same batch row for row)."""
+    d, N = student.distillation, student.batch
+    t = d.teacher
+    student._e.softmax_kd_head(student.logits16, student.p("fc.bias"), t.logits16, t.p("fc.bias"), student.labels, mix,
+                               student.label_smoothing, d.alpha, d.temperature, student.logits, dlogits16,
+                               student.loss_rows, student.stats, 1.0 / N)
+
+
 def resnet50_blocks(image_size: int = 224) -> List[BlockSpec]:
     cfg = [(64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)]
     blocks = []
@@ -109,6 +136,8 @@ class ResNet50Engine:
         self._augmenter = None
         # Keras's label smoothing of the loss; the Trainer sets it from the compiled loss before capturing the steps
         self.label_smoothing = 0.0
+        self.distillation = None   # `train.losses.Distillation` with an engine teacher: set by `set_distillation`
+        self._teacher_in: Optional[torch.Tensor] = None   # a student's stem input this engine reads as a teacher
         self.zero_init_residual = zero_init_residual
         self.native_stem = native_stem
         # experimental: run every weight-gradient GEMM on a side stream so it overlaps the (DRAM-bound) BatchNorm
@@ -306,7 +335,8 @@ class ResNet50Engine:
         # training steps read the augmented copy of x_u8 (every stem reader below); eval reads x_u8 itself
         self._augmenter = _augmenter(self, self.x_u8) if training else None
         x_train = self._augmenter.out if self._augmenter is not None else self.x_u8
-        self.stats = torch.zeros(2, **f32)          # [sum loss, correct]
+        # [sum loss, correct] (+ [sum student loss, sum distillation loss] when distilling)
+        self.stats = torch.zeros(_stats_len(self), **f32)
         self.logits = torch.zeros(N, self.num_classes, **f32)  # fp32 logits (+bias) for predict(); written by the CE kernel
         self.loss_rows = torch.zeros(N, **f32)
 
@@ -338,6 +368,8 @@ class ResNet50Engine:
             self._stem_fwd = C.StemForward(self.x_u8, self._stem_w16, self.y0, w0["sum"], w0["sqsum"], max_ctas=self.max_ctas)
             self._stem_fwd_train = self._stem_fwd if x_train is self.x_u8 else \
                 C.StemForward(x_train, self._stem_w16, self.y0, w0["sum"], w0["sqsum"], max_ctas=self.max_ctas)
+            self._stem_fwd_teacher = None if self._teacher_in is None else \
+                C.StemForward(self._teacher_in, self._stem_w16, self.y0, w0["sum"], w0["sqsum"], max_ctas=self.max_ctas)
         else:
             self._stem_w = torch.zeros(64, 3, 7, 7, **bf).contiguous(memory_format=torch.channels_last)
         self._refresh_stem_weight()
@@ -562,6 +594,8 @@ class ResNet50Engine:
         self._training_built = training
         self._built = True
         self.sync_weights()
+        if training and self.distillation is not None:
+            self.distillation.teacher.bind_teacher_input(self._stem_input(True))
         return self
 
     # ------------------------------------------------------------------------------------------------ forward
@@ -598,6 +632,13 @@ class ResNet50Engine:
 
     def forward(self, training: bool = True) -> None:
         """x_u8 / labels (static inputs) -> logits, loss stats.  All launches go to the current stream."""
+        self.forward_logits(training)
+        self.forward_head(training)
+
+    def forward_logits(self, training: bool = True, teacher: bool = False) -> None:
+        """Augmentation (training), a distillation teacher's logits (training), features and the bf16 FC logits
+        ``logits16``.  ``teacher=True``: the inference forward of this engine as a distillation teacher, reading the
+        student's stem input bound by `bind_teacher_input` instead of ``x_u8``."""
         e, N, A = self._e, self.batch, self.act
         w0 = self.bnw["bn1"]
         if self._tail_plans and self._tail_state != training:
@@ -611,11 +652,15 @@ class ResNet50Engine:
         augment = training and self._augmenter is not None
         if augment:
             self._augmenter.run()
+        if training and self.distillation is not None:
+            # the teacher reads this step's stem input in place, before the stem: its logits16 feed the head
+            self.distillation.teacher.forward_logits(False, teacher=True)
         if self.native_stem:
             # 7x7/2 stem on the tensor cores straight from the uint8 batch (normalisation + BN statistics fused)
-            (self._stem_fwd_train if training else self._stem_fwd).run()
+            (self._stem_fwd_teacher if teacher else self._stem_fwd_train if training else self._stem_fwd).run()
         else:
-            e.preprocess_u8(self._augmenter.out if augment else self.x_u8, self.x16, 1.0 / 127.5, -1.0)
+            src = self._teacher_in if teacher else self._augmenter.out if augment else self.x_u8
+            e.preprocess_u8(src, self.x16, 1.0 / 127.5, -1.0)
             y0 = torch.nn.functional.conv2d(self.x16.permute(0, 3, 1, 2), self._stem_w, stride=2, padding=3)
             self.y0.copy_(y0.permute(0, 2, 3, 1))
             e.channel_stats(self.y0, w0["sum"], w0["sqsum"])
@@ -653,17 +698,22 @@ class ResNet50Engine:
         self._drop_seed = self.seed * 1000003 + self._step_count
         e.gap_fwd(self.feat, self.pooled, drop, self._drop_seed)
         self._fc_fwd.run()  # bf16 logits (class dimension padded) on the wgmma GEMM
+
+    def forward_head(self, training: bool = True) -> None:
+        """+ bias, softmax cross-entropy, accuracy, bf16 dlogits (padded columns zero) in one kernel; against the soft
+        target when the batch is mixed or the labels smoothed, plus the teacher's term when distilling."""
+        e, N = self._e, self.batch
         e.zero_(self.stats)
-        # + bias, softmax cross-entropy, accuracy, bf16 dlogits (padded columns zero) in one kernel; against the soft
-        # target when the batch is mixed or the labels smoothed
         mix = self._augmenter.mix if (training and self._augmenter is not None) else None
-        if mix is None and self.label_smoothing == 0:
-            e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits,
-                              self.dlogits16 if training else None, self.loss_rows, self.stats, 1.0 / N)
+        dl = self.dlogits16 if training else None
+        if training and self.distillation is not None:
+            _kd_head(self, mix, dl)
+        elif mix is None and self.label_smoothing == 0:
+            e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits, dl, self.loss_rows,
+                              self.stats, 1.0 / N)
         else:   # soft targets: the partner's label at the mix row's weight, label smoothing
             e.softmax_ce_soft_head(self.logits16, self.p("fc.bias"), self.labels, mix, self.label_smoothing,
-                                   self.logits, self.dlogits16 if training else None, self.loss_rows, self.stats,
-                                   1.0 / N)
+                                   self.logits, dl, self.loss_rows, self.stats, 1.0 / N)
 
     # ------------------------------------------------------------------------------------------------ backward
     def _ready(self, *names: str) -> None:
@@ -838,6 +888,26 @@ class ResNet50Engine:
         if self._augmenter is not None:
             self._augmenter.set_step(t)
 
+    def set_distillation(self, distillation) -> None:
+        """Distil from ``distillation.teacher`` (a `train.losses.Distillation`; None: plain training) in the training
+        steps captured from now on (see the module-level `set_distillation`)."""
+        set_distillation(self, distillation)
+
+    def bind_teacher_input(self, x_u8: torch.Tensor) -> None:
+        """Teach a student whose stem reads ``x_u8``: build for inference if not built (as `EngineEvalStep` does) and
+        add one stem binding to that buffer, read by ``forward_logits(training=False, teacher=True)``."""
+        self._teacher_in = x_u8
+        if not self._built:
+            self.build(training=self.grads is not None)   # binds the stem to x_u8 too
+        elif self.native_stem:
+            w0 = self.bnw["bn1"]
+            self._stem_fwd_teacher = C.StemForward(x_u8, self._stem_w16, self.y0, w0["sum"], w0["sqsum"],
+                                                   max_ctas=self.max_ctas)
+
+    def _stem_input(self, training: bool) -> torch.Tensor:
+        """uint8 batch the stem reads: the augmented copy in training steps, x_u8 otherwise."""
+        return self._augmenter.out if (training and self._augmenter is not None) else self.x_u8
+
     def loss_and_acc(self) -> Tuple[float, float]:
         s = self.stats.tolist()
         return s[0] / self.batch, s[1] / self.batch
@@ -926,7 +996,7 @@ class EngineTrainStep:
         if self._dist:
             optimizer.extra_wait_streams = list(e.aux_streams)
         self._warmup_steps = warmup_steps
-        self._host_stats = torch.zeros(2, dtype=torch.float32).pin_memory()
+        self._host_stats = torch.zeros(e.stats.numel(), dtype=torch.float32).pin_memory()
         self.steps = 0
         self._captured = False
 
@@ -1032,7 +1102,7 @@ class EngineEvalStep:
         self.use_graph = use_graph
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         engine.build(training=engine.grads is not None)
-        self._host_stats = torch.zeros(2, dtype=torch.float32).pin_memory()
+        self._host_stats = torch.zeros(engine.stats.numel(), dtype=torch.float32).pin_memory()
 
     def capture(self) -> None:
         e = self.engine

@@ -4,8 +4,8 @@ from .callbacks import (Callback, History, EarlyStopping, ReduceLROnPlateau, Mod
 from .trainer import Trainer
 from .flat import FlatParams
 from . import callbacks, losses
-from .losses import CategoricalCrossentropy, SparseCategoricalCrossentropy
+from .losses import CategoricalCrossentropy, Distillation, SparseCategoricalCrossentropy
 
 __all__ = ["Trainer", "Callback", "History", "EarlyStopping", "ReduceLROnPlateau", "ModelCheckpoint",
            "LambdaCallback", "CallbackList", "FlatParams", "losses", "callbacks", "SparseCategoricalCrossentropy",
-           "CategoricalCrossentropy"]
+           "CategoricalCrossentropy", "Distillation"]

@@ -28,12 +28,13 @@ def _is_engine(model) -> bool:
 
 
 class _EngineBackend:
-    def __init__(self, engine, optimizer, use_graph: bool, label_smoothing: float = 0.0):
-        from ..models.resnet_engine import EngineTrainStep, EngineEvalStep
+    def __init__(self, engine, optimizer, use_graph: bool, label_smoothing: float = 0.0, distillation=None):
+        from ..models.resnet_engine import _stats_len
 
         self.engine = engine
         # read by the head of every forward: set before the (lazily built) steps capture their graphs
         engine.label_smoothing = float(label_smoothing)
+        engine.set_distillation(distillation)
         self.optimizer = optimizer
         self.use_graph = use_graph
         # Both step objects are created on first use: a Trainer that only ever predicts (pyfunc serving, load_model) builds
@@ -45,8 +46,10 @@ class _EngineBackend:
         self.batch = engine.batch
         self._pending = deque()
         # one pinned result slot per IN-FLIGHT step: a slot goes back to the free list only after its value has been
-        # read, so queueing many batches before popping (evaluate) can never overwrite an unread result
-        self._free = [torch.zeros(2, dtype=torch.float32).pin_memory() for _ in range(4)]
+        # read, so queueing many batches before popping (evaluate) can never overwrite an unread result.  Four floats
+        # when distilling: training steps also report the student and distillation terms.
+        self._slot = _stats_len(engine)
+        self._free = [torch.zeros(self._slot, dtype=torch.float32).pin_memory() for _ in range(4)]
 
     @property
     def step(self):
@@ -67,26 +70,27 @@ class _EngineBackend:
             self._eval_step = EngineEvalStep(self.engine, use_graph=self.use_graph)
         return self._eval_step
 
-    def _enqueue_result(self) -> None:
-        buf = self._free.pop() if self._free else torch.zeros(2, dtype=torch.float32).pin_memory()
-        buf.copy_(self.engine.stats, non_blocking=True)
+    def _enqueue_result(self, n: int = 2) -> None:
+        buf = self._free.pop() if self._free else torch.zeros(self._slot, dtype=torch.float32).pin_memory()
+        buf[:n].copy_(self.engine.stats[:n], non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        self._pending.append((ev, buf))
+        self._pending.append((ev, buf, n))
 
-    def pop_results(self, keep: int = 0) -> List[Tuple[float, float]]:
+    def pop_results(self, keep: int = 0) -> List[Tuple[float, ...]]:
+        """(loss, accuracy) per step, + (student loss, distillation loss) for a distilling training step."""
         out = []
         while len(self._pending) > keep:
-            ev, buf = self._pending.popleft()
+            ev, buf, n = self._pending.popleft()
             ev.synchronize()
-            out.append((float(buf[0]) / self.batch, float(buf[1]) / self.batch))
+            out.append(tuple(float(v) / self.batch for v in buf[:n]))
             self._free.append(buf)
         return out
 
     def train_batch(self, x, y) -> None:
         self.step.load(x, y)
         self.step.run()
-        self._enqueue_result()
+        self._enqueue_result(self._slot)
 
     def eval_batch(self, x, y) -> None:
         step = self.eval_step  # (builds the engine on first use)
@@ -167,9 +171,12 @@ class _EngineBackend:
 
 class _ModuleBackend:
     def __init__(self, module: torch.nn.Module, optimizer, preprocess, device: torch.device,
-                 label_smoothing: float = 0.0):
+                 label_smoothing: float = 0.0, distillation=None):
         self.module = module.to(device)
         self.label_smoothing = float(label_smoothing)
+        self.distillation = distillation
+        if distillation is not None:
+            distillation.teacher.to(device)
         self.device = device
         self.optimizer = optimizer
         self.preprocess = preprocess
@@ -203,7 +210,7 @@ class _ModuleBackend:
         return augment_batch_reference(self.module.augmentation, x.to(self.device, non_blocking=True), key, opt.t)
 
     def train_batch(self, x, y) -> None:
-        from ..models.augment import soft_targets, target_argmax
+        from ..models.augment import distillation_reference, soft_targets, target_argmax
 
         self.module.train()
         y = torch.as_tensor(y).to(self.device, non_blocking=True)
@@ -214,8 +221,21 @@ class _ModuleBackend:
         self.flat.zero_grad()
         if self._dist:
             self.optimizer.start_backward()
+        d = self.distillation
+        if d is not None:   # the frozen teacher, in inference mode, on the batch the student sees
+            d.teacher.eval()
+            with torch.no_grad():
+                t_logits = d.teacher(self._prep(x)).float()
         logits = self.module(self._prep(x)).float()
         eps = self.label_smoothing
+        if d is not None:
+            rows = distillation_reference(logits, t_logits, y, mix, eps, d.alpha, d.temperature)
+            loss, ce, kd = (r.mean() for r in rows)
+            acc = (logits.argmax(1) == target_argmax(y, mix)).float().mean()
+            loss.backward()
+            self.optimizer.step()
+            self._results.append(torch.stack([loss.detach(), acc, ce.detach(), kd.detach()]))
+            return
         if mix is None and eps == 0:
             loss = torch.nn.functional.cross_entropy(logits, y)
             acc = (logits.argmax(1) == y).float().mean()
@@ -240,11 +260,11 @@ class _ModuleBackend:
         self.module.eval()
         return self.module(self._prep(x)).float()
 
-    def pop_results(self, keep: int = 0) -> List[Tuple[float, float]]:
+    def pop_results(self, keep: int = 0) -> List[Tuple[float, ...]]:
+        """(loss, accuracy) per step, + (student loss, distillation loss) for a distilling training step."""
         out = []
         while len(self._results) > keep:
-            t = self._results.popleft().tolist()
-            out.append((t[0], t[1]))
+            out.append(tuple(self._results.popleft().tolist()))
         return out
 
     def state_tensors(self) -> List[torch.Tensor]:
@@ -277,6 +297,7 @@ class Trainer:
         self.use_graph = use_graph
         self.optimizer = None
         self.backend = None
+        self.distillation = None   # the compiled `losses.Distillation`, if any
         self.metrics_names = ["loss"]
         self.stop_training = False
         self.steps_per_epoch: Optional[int] = None
@@ -294,20 +315,24 @@ class Trainer:
             from .. import optim
 
             optimizer = optim.get(optimizer)()
-        from .losses import CategoricalCrossentropy, label_smoothing_of
+        from .losses import CategoricalCrossentropy, Distillation, label_smoothing_of
 
         eps = label_smoothing_of(loss)
         aug = getattr(self.model, "augmentation", None)
-        if aug is not None and aug.mix_mode and not (isinstance(loss, CategoricalCrossentropy)
+        if aug is not None and aug.mix_mode and not (isinstance(loss, (CategoricalCrossentropy, Distillation))
                                                      or loss == "categorical_crossentropy"):
             raise ValueError("MixUp / CutMix train on soft targets: compile with "
                              "CategoricalCrossentropy(from_logits=True) or 'categorical_crossentropy'")
+        distill = loss if isinstance(loss, Distillation) else None
+        if distill is not None:
+            distill.check_student(self.model)
         self.optimizer = optimizer
         self.metrics_names = ["loss"] + [m if isinstance(m, str) else getattr(m, "name", "metric") for m in metrics]
         if _is_engine(self.model):
-            self.backend = _EngineBackend(self.model, optimizer, self.use_graph, eps)
+            self.backend = _EngineBackend(self.model, optimizer, self.use_graph, eps, distill)
         else:
-            self.backend = _ModuleBackend(self.model, optimizer, self._preprocess, self.device, eps)
+            self.backend = _ModuleBackend(self.model, optimizer, self._preprocess, self.device, eps, distill)
+        self.distillation = distill
         return self
 
     # ------------------------------------------------------------------------------------------------ fit
@@ -329,7 +354,7 @@ class Trainer:
         for epoch in range(initial_epoch, epochs):
             cbs.call("on_epoch_begin", epoch, {})
             t0 = time.perf_counter()
-            tot_loss = tot_acc = 0.0
+            tot = [0.0] * 4   # loss, accuracy, student loss, distillation loss
             n_seen = 0
             for b in range(steps_per_epoch):
                 cbs.call("on_train_batch_begin", b, {})
@@ -343,19 +368,22 @@ class Trainer:
                         raise ValueError("fit(): the dataset yields no batches (fewer rows than batch_size?)") from None
                 self.backend.train_batch(xb, yb)
                 steps_run += 1
-                for l, a in self.backend.pop_results(keep=1):  # lag one step: keeps H2D/compute overlapped
-                    tot_loss += l
-                    tot_acc += a
+                for r in self.backend.pop_results(keep=1):  # lag one step: keeps H2D/compute overlapped
+                    for i, v in enumerate(r):
+                        tot[i] += v
                     n_seen += 1
                 cbs.call("on_train_batch_end", b, {})
-            for l, a in self.backend.pop_results(keep=0):
-                tot_loss += l
-                tot_acc += a
+            for r in self.backend.pop_results(keep=0):
+                for i, v in enumerate(r):
+                    tot[i] += v
                 n_seen += 1
             dt = time.perf_counter() - t0
-            logs: Dict[str, float] = {"loss": tot_loss / max(n_seen, 1)}
+            logs: Dict[str, float] = {"loss": tot[0] / max(n_seen, 1)}
             if "accuracy" in self.metrics_names:
-                logs["accuracy"] = tot_acc / max(n_seen, 1)
+                logs["accuracy"] = tot[1] / max(n_seen, 1)
+            if self.distillation is not None:   # the two terms of the Keras example's Distiller
+                logs["student_loss"] = tot[2] / max(n_seen, 1)
+                logs["distillation_loss"] = tot[3] / max(n_seen, 1)
             bsz = self._batch_size(xb)
             logs["images_per_sec"] = steps_per_epoch * bsz * dist_core.size() / max(dt, 1e-9)
             if validation_data is not None:
@@ -456,10 +484,22 @@ class Trainer:
 
     # ------------------------------------------------------------------------------------------------ state
     def broadcast_state(self, root: int = 0) -> None:
-        """K2: identical weights / optimizer state / BN statistics on every rank."""
+        """K2: identical weights / optimizer state / BN statistics on every rank - and a distillation teacher's weights
+        and statistics (in Keras the teacher is a sub-model of the ``Distiller``, which the broadcast covers)."""
         for t in self.backend.state_tensors():
             dist_core.broadcast(t, root)
         self.backend.after_state_change()
+        if self.distillation is not None:
+            teacher = self.distillation.teacher
+            if _is_engine(teacher):
+                # through the state dict: a frozen MobileNetV2 base keeps its weights outside the flat parameters
+                sd = {k: v.to(teacher.device) for k, v in teacher.state_dict().items()}
+                for v in sd.values():
+                    dist_core.broadcast(v, root)
+                teacher.load_state_dict(sd)
+            else:
+                for v in teacher.state_dict().values():   # parameters and buffers, in place
+                    dist_core.broadcast(v, root)
 
     def get_weights(self):
         return self.backend.state_dict()
