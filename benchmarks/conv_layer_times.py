@@ -82,14 +82,8 @@ def dgrad_part_pixels(dg: ConvDgrad, N: int):
     return px
 
 
-def main() -> None:
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--batch", type=int, default=256)
-    ap.add_argument("--iters", type=int, default=25)
-    ap.add_argument("--json", default=None, help="also write the rows as JSON to this path")
-    args = ap.parse_args()
-    assert torch.cuda.is_available(), "conv_layer_times.py needs a GPU"
-    N = args.batch
+def trained_engine(N: int) -> ResNet50Engine:
+    """A training ``ResNet50Engine(batch=N)`` after two eager steps, so every buffer holds step-like data."""
     eng = ResNet50Engine(batch=N, num_classes=1000, seed=0)
     step = EngineTrainStep(eng, optim.SGD(0.1, momentum=0.9), use_graph=False)
     g = torch.Generator(device="cuda").manual_seed(0)
@@ -98,16 +92,14 @@ def main() -> None:
     for _ in range(2):
         step.run()
     torch.cuda.synchronize()
+    return eng
 
+
+def dgrad_jobs(eng: ResNet50Engine, N: int):
+    """(layer, kind, plan, flops, bytes, k-blocks per tile) of every data-gradient launch of the residual blocks."""
     shapes = conv_shapes(N)
     blocks = {b.name: b for b in resnet50_blocks()}
-    jobs = []  # (layer, kind, plan, flops, bytes, k-blocks per tile)
-    for name, op in eng._fwd.items():
-        R, s, hi, ho, ci, co = shapes[name]
-        a_px = N * ho * ho if (R == 1 and s > 1) else N * hi * hi  # a strided 1x1 conv reads only its sampled pixels
-        flops = 2.0 * N * ho * ho * co * ci * R * R
-        nbytes = 2.0 * (a_px * ci + R * R * co * ci + N * ho * ho * co)
-        jobs.append((name, "fwd", op.plan, flops, nbytes, R * R * (-(-ci // 64))))
+    jobs = []
     for name, dg in eng._dg.items():
         R, s, hi, ho, ci, co = shapes[name]
         dy_elems = N * ho * ho * co
@@ -122,6 +114,27 @@ def main() -> None:
                 nbytes += 2.0 * skip_px * ci + px * ci / 8 + 2.0 * px * ci  # skip gradient, ReLU bit mask, y3
             kind = "dgrad" if len(dg.parts) == 1 else f"dgrad[{len(idx)}taps]"
             jobs.append((name, kind, plan, flops, nbytes, len(idx) * (-(-co // 64))))
+    return jobs
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--iters", type=int, default=25)
+    ap.add_argument("--json", default=None, help="also write the rows as JSON to this path")
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "conv_layer_times.py needs a GPU"
+    N = args.batch
+    eng = trained_engine(N)
+    shapes = conv_shapes(N)
+    jobs = []  # (layer, kind, plan, flops, bytes, k-blocks per tile)
+    for name, op in eng._fwd.items():
+        R, s, hi, ho, ci, co = shapes[name]
+        a_px = N * ho * ho if (R == 1 and s > 1) else N * hi * hi  # a strided 1x1 conv reads only its sampled pixels
+        flops = 2.0 * N * ho * ho * co * ci * R * R
+        nbytes = 2.0 * (a_px * ci + R * R * co * ci + N * ho * ho * co)
+        jobs.append((name, "fwd", op.plan, flops, nbytes, R * R * (-(-ci // 64))))
+    jobs += dgrad_jobs(eng, N)
     ncp = eng.classes_padded
     jobs.append(("fc", "fwd", eng._fc_fwd.plan, 2.0 * N * 2048 * ncp, 2.0 * (N * 2048 + ncp * 2048 + N * ncp), 2048 // 64))
     for plan, _, _ in eng._fc_dg.parts:

@@ -117,6 +117,14 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
   constexpr bool kAffine = kStats == 4;                  // epilogue: acc*scale + shift (+ residual) -> activation
   constexpr int kChunks = BLOCK_N / 64;
   constexpr int kAcc = BLOCK_N / 2;                      // fp32 accumulators per thread and 64-row half of the tile
+  // kStats == 3: chunk 0's skip-gradient and mask words are loaded while the tile's last MMAs drain.  At BLOCK_N = 128
+  // their 40 registers beside the 128 accumulators would spill, so that tile loads chunk 0 row by row in the epilogue.
+  constexpr bool kSkipEarly = BLOCK_N == 64;
+  // kHasY: chunk 0's pre-BN tile is requested when the warpgroup starts the tile's main loop, instead of after it.  This
+  // pays where the main loop is short next to the epilogue (kStats == 3: 1-8 k-blocks per tile) and on the BLOCK_N = 64
+  // plans; the long main loops of the BLOCK_N = 128 kStats == 2 plans hide the load already, and there the early
+  // request measured slower, so they keep the epilogue's request.
+  constexpr bool kEarlyY = kHasY && (kStats == 3 || BLOCK_N == 64);
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = align_smem_1024(smem_raw);
@@ -284,7 +292,8 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
 
     // kStats == 3 / kAffine residual: this thread's four rows of the additive tensor (flat mode: tile row == pixel
     // index), row r16 + 8 * (q & 1) + 64 * (q >> 1) for q = 2 * mh + h.  Computed before the main loop (scalar work
-    // the MMAs hide); the loads themselves sit in the epilogue, under the other warpgroup's MMAs.
+    // the MMAs hide).  The loads sit in the epilogue, under the other warpgroup's MMAs, except where kStats == 3 issues
+    // them earlier (skip_ld below).
     const __nv_bfloat16* arow[4] = {nullptr, nullptr, nullptr, nullptr};
     const uint8_t* mrow[4] = {nullptr, nullptr, nullptr, nullptr};
     if ((kStats == 3 || kAffine) && p.mode == 0 && (kStats == 3 || p.add_src != nullptr)) {
@@ -307,11 +316,36 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
         }
       }
     }
+    // kStats == 3: row q's skip-gradient words and ReLU-mask bits of one chunk, all issued before any is used (one
+    // memory latency per row, not per 8-column group).  skg[q][j]: columns 8j + cq, cq + 1; skm[q]: bit k of byte j =
+    // column 8j + k.  Chunk c + 1's are issued once chunk c is staged, chunk 0's before wgmma_wait<0> (kSkipEarly).
+    uint32_t skg[4][8];
+    uint64_t skm[4];
+    auto skip_ld = [&](int q, int c) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        skg[q][j] = arow[q] != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(arow[q] + c * 64 + j * 8 + cq)) : 0u;
+      skm[q] = mrow[q] != nullptr ? __ldg(reinterpret_cast<const unsigned long long*>(mrow[q] + c * 8)) : 0ull;
+    };
+    // kHasY: the pre-BN tile of chunk c into sYW (one per warpgroup), by the warpgroup's thread 0
+    auto y_ld = [&](int c) {
+      mbar_arrive_expect_tx(&y_bar[wg], static_cast<uint32_t>(p.valid_rows) * 128u);
+      if (p.mode == 0)
+        tma_load_2d(sYW, &tmY, &y_bar[wg], nb * BLOCK_N + c * 64, m_tile * kBlockM);
+      else
+        tma_load_4d(sYW, &tmY, &y_bar[wg], nb * BLOCK_N + c * 64, w0, h0, n0);
+    };
     // ---------------------------------------------------------------- main loop
     // One stage = one k-block (or, in halo mode, three vertical taps of one k-block).  The MMAs of a stage stay in
     // flight while the next stage is waited for; a stage is released once the group after it has been issued.
     // The other warpgroup has issued all MMAs of the previous tile (so every stage before this tile's is filled).
     if (i > 0) named_bar_sync(my_turn, kConvConsumers);
+    if (kEarlyY) {
+      // Chunk 0's pre-BN tile lands during the main loop.  This barrier stands in for chunk 0's epilogue barrier.
+      if (wtid == 0) tma_store_wait_read<kChunks - 1>();  // the store from staging buffer 0 one tile ago has read it
+      named_bar_sync(epi_bar, 128);  // the previous tile's statistics are done reading sYW and the staging buffers
+      if (wtid == 0) y_ld(0);
+    }
     float acc[2][kAcc];
 #pragma unroll
     for (int mh = 0; mh < 2; ++mh)
@@ -352,6 +386,10 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
     }
     // every stage of this tile has been waited for: the other warpgroup may start its tile while these MMAs drain
     if (tile + static_cast<int>(gridDim.x) < p.num_tiles) named_bar_arrive(their_turn, kConvConsumers);
+    if (kStats == 3 && kSkipEarly) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) skip_ld(q, 0);
+    }
     wgmma_wait<0>();
     fence_acc(acc[0]);
     fence_acc(acc[1]);
@@ -364,30 +402,30 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
 #pragma unroll
     for (int c = 0; c < kChunks; ++c, ++chunk_ctr) {
       uint8_t* sbuf = sStageW + c * kTileChunkBytes;
-      if (wtid == 0) tma_store_wait_read<kChunks - 1>();  // the store from this buffer one tile ago has read it
-      named_bar_sync(epi_bar, 128);                        // ... and the warpgroup is done with its statistics
-      if (kHasY && wtid == 0) {
-        // pre-BN tile of this chunk (the previous chunk's readers are done: barrier above)
-        mbar_arrive_expect_tx(&y_bar[wg], static_cast<uint32_t>(p.valid_rows) * 128u);
-        if (p.mode == 0)
-          tma_load_2d(sYW, &tmY, &y_bar[wg], nb * BLOCK_N + c * 64, m_tile * kBlockM);
-        else
-          tma_load_4d(sYW, &tmY, &y_bar[wg], nb * BLOCK_N + c * 64, w0, h0, n0);
+      if (!kEarlyY || c > 0) {  // kEarlyY chunk 0: the barrier before the main loop
+        if (wtid == 0) tma_store_wait_read<kChunks - 1>();  // the store from this buffer one tile ago has read it
+        named_bar_sync(epi_bar, 128);  // the store has read this buffer and the statistics are done with it and sYW
       }
+      if (kHasY && (c > 0 || !kEarlyY) && wtid == 0) y_ld(c);  // the last statistics are done with sYW: barrier above
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const int mh = q >> 1, h = q & 1;
         const int row = 64 * mh + r16 + 8 * h;
-        // This row's residual / skip-gradient words and ReLU-mask bits, all issued before any is used: one memory
-        // latency per row instead of one per 8-column group (the smem stores below would otherwise keep the compiler
-        // from hoisting the loads).  gv[j]: columns 8j + cq, cq + 1; mv: bit k of byte j = column 8j + k.
+        // This row's residual / skip-gradient words and ReLU-mask bits.  kAffine issues all of its residual loads
+        // before any is used: one memory latency per row instead of one per 8-column group (the smem stores below would
+        // otherwise keep the compiler from hoisting the loads).  gv[j]: columns 8j + cq, cq + 1; mv: bit k of byte j =
+        // column 8j + k.
         uint32_t gv[8];
         uint64_t mv = 0ull;
-        if (kStats == 3 || kAffine) {
+        if (kStats == 3) {
+          if (c == 0 && !kSkipEarly) skip_ld(q, 0);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) gv[j] = skg[q][j];
+          mv = skm[q];
+        } else if (kAffine) {
 #pragma unroll
           for (int j = 0; j < 8; ++j)
             gv[j] = arow[q] != nullptr ? __ldg(reinterpret_cast<const unsigned int*>(arow[q] + c * 64 + j * 8 + cq)) : 0u;
-          if (kStats == 3 && mrow[q] != nullptr) mv = __ldg(reinterpret_cast<const unsigned long long*>(mrow[q] + c * 8));
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -415,8 +453,12 @@ conv_igemm_kernel(const __grid_constant__ TmapArray4 tmA, const __grid_constant_
           *reinterpret_cast<uint32_t*>(sbuf + row * 128 + ((j ^ (row & 7)) << 4) + (lane & 3) * 4) = w;
         }
       }
+      if (kStats == 3 && c + 1 < kChunks) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) skip_ld(q, c + 1);  // next chunk's rows, in flight from here on
+      }
       fence_proxy_async_smem();
-      named_bar_sync(epi_bar, 128);
+      named_bar_sync(epi_bar, 128);  // every staging write is done before the TMA store and the statistics read them
       if (wtid == 0) {
         const int ccol = nb * BLOCK_N + c * 64;
         if (p.mode == 0)
