@@ -413,6 +413,9 @@ void bn_bwd_reduce(int mode, const void* g1, const void* g2, const void* outp, c
 
 // ------------------------------------------------------------------------------------------------ BN bwd coeffs
 // dy = A*dz + B*y + Cc   with  A = gamma*invstd,  B = -A*invstd*dgamma/M,  Cc = -A*dbeta/M - B*mean
+// kInference: BatchNorm normalised with its running statistics (mean / invstd are the running ones), so the batch
+// statistics carry no gradient: B = Cc = 0 and dy = A*dz.  dgamma / dbeta are the same expressions in both modes.
+template <bool kInference>
 __global__ void bn_bwd_coeffs_kernel(float* __restrict__ sum_dz, float* __restrict__ sum_dzy,
                                      const float* __restrict__ gamma, const float* __restrict__ mean,
                                      const float* __restrict__ invstd, float inv_count, float* __restrict__ dgamma,
@@ -429,16 +432,22 @@ __global__ void bn_bwd_coeffs_kernel(float* __restrict__ sum_dz, float* __restri
   dgamma[c] = dg;
   dbeta[c] = db;
   const float A = gamma[c] * is;
-  const float B = -A * is * dg * inv_count;
   cA[c] = A;
-  cB[c] = B;
-  cC[c] = -A * db * inv_count - B * m;
+  if (kInference) {
+    cB[c] = 0.f;
+    cC[c] = 0.f;
+  } else {
+    const float B = -A * is * dg * inv_count;
+    cB[c] = B;
+    cC[c] = -A * db * inv_count - B * m;
+  }
 }
 void bn_bwd_coeffs(float* sum_dz, float* sum_dzy, const float* gamma, const float* mean, const float* invstd,
-                   double count, float* dgamma, float* dbeta, float* cA, float* cB, float* cC, int C,
+                   double count, float* dgamma, float* dbeta, float* cA, float* cB, float* cC, int C, bool inference,
                    cudaStream_t s) {
-  bn_bwd_coeffs_kernel<<<(C + 127) / 128, 128, 0, s>>>(sum_dz, sum_dzy, gamma, mean, invstd, (float)(1.0 / count),
-                                                        dgamma, dbeta, cA, cB, cC, C);
+  auto kernel = inference ? bn_bwd_coeffs_kernel<true> : bn_bwd_coeffs_kernel<false>;
+  kernel<<<(C + 127) / 128, 128, 0, s>>>(sum_dz, sum_dzy, gamma, mean, invstd, (float)(1.0 / count), dgamma, dbeta,
+                                          cA, cB, cC, C);
 }
 
 // dy = A*dz + B*y + Cc  with dz either read as-is (MASK=false: stored dz / BN without ReLU) or recomputed as

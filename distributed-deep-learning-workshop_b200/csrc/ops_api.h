@@ -46,7 +46,8 @@ void channel_stats(const void* y, float* sum, float* sqsum, int64_t M, int C, cu
 void bn_bwd_reduce(int mode, const void* g1, const void* g2, const void* outp, const void* y, const float* scale,
                    const float* shift, void* dz_out, float* sum_dz, float* sum_dzy, int64_t M, int C, cudaStream_t s);
 void bn_bwd_coeffs(float* sum_dz, float* sum_dzy, const float* gamma, const float* mean, const float* invstd,
-                   double count, float* dgamma, float* dbeta, float* cA, float* cB, float* cC, int C, cudaStream_t s);
+                   double count, float* dgamma, float* dbeta, float* cA, float* cB, float* cC, int C, bool inference,
+                   cudaStream_t s);
 void bn_bwd_apply(const void* g, const void* y, const float* scale, const float* shift, const float* cA,
                   const float* cB, const float* cC, void* dy, int64_t M, int C, cudaStream_t s);
 void maxpool_fwd(const void* x, void* out, void* idx, int N, int H, int W, int C, cudaStream_t s);

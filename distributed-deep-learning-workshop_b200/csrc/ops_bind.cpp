@@ -123,8 +123,9 @@ void bn_bwd_reduce(int64_t mode, Tensor g1, OptT g2, OptT outp, Tensor y, OptT s
   after();
 }
 
+// inference: the BatchNorm normalised with its running statistics (mean / invstd): B = C = 0, dy = A * dz
 void bn_bwd_coeffs(Tensor sum_dz, Tensor sum_dzy, Tensor gamma, Tensor mean, Tensor invstd, double count,
-                   Tensor dgamma, Tensor dbeta, Tensor cA, Tensor cB, Tensor cC) {
+                   Tensor dgamma, Tensor dbeta, Tensor cA, Tensor cB, Tensor cC, bool inference) {
   const int C = (int)gamma.numel();
   for (const auto& [t, name] : {std::pair<const Tensor*, const char*>{&sum_dz, "sum_dz"}, {&sum_dzy, "sum_dzy"},
                                 {&gamma, "gamma"}, {&mean, "mean"}, {&invstd, "invstd"}, {&dgamma, "dgamma"},
@@ -133,7 +134,7 @@ void bn_bwd_coeffs(Tensor sum_dz, Tensor sum_dzy, Tensor gamma, Tensor mean, Ten
   b200::bn_bwd_coeffs(sum_dz.data_ptr<float>(), sum_dzy.data_ptr<float>(), gamma.data_ptr<float>(),
                       mean.data_ptr<float>(), invstd.data_ptr<float>(), count, dgamma.data_ptr<float>(),
                       dbeta.data_ptr<float>(), cA.data_ptr<float>(), cB.data_ptr<float>(), cC.data_ptr<float>(), C,
-                      cur());
+                      inference, cur());
   after();
 }
 
@@ -949,7 +950,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("mask") = c10::nullopt, py::arg("relu6") = false);
   m.def("channel_stats", &channel_stats);
   m.def("bn_bwd_reduce", &bn_bwd_reduce);
-  m.def("bn_bwd_coeffs", &bn_bwd_coeffs);
+  m.def("bn_bwd_coeffs", &bn_bwd_coeffs, py::arg("sum_dz"), py::arg("sum_dzy"), py::arg("gamma"), py::arg("mean"),
+        py::arg("invstd"), py::arg("count"), py::arg("dgamma"), py::arg("dbeta"), py::arg("cA"), py::arg("cB"),
+        py::arg("cC"), py::arg("inference") = false);
   m.def("bn_bwd_apply", &bn_bwd_apply);
   m.def("bn_apply_fused", &bn_apply_fused, py::arg("y"), py::arg("pack"), py::arg("count"), py::arg("momentum"),
         py::arg("eps"), py::arg("res") = c10::nullopt, py::arg("res_pack") = c10::nullopt, py::arg("out"),

@@ -9,6 +9,8 @@
 `MobileNetV2Engine` (depthwise / stem kernels + wgmma pointwise convs with folded-BN epilogues), on CPU (or with
 `arch='mobilenetv2_torch'`, or `freeze_base=False`) the torch.nn module.
 `arch='resnet50_torch'`: torchvision-architecture ResNet-50 as a plain nn.Module (CPU plumbing runs).
+`arch='resnet50_head'`: ResNet-50 base + GAP + Dropout + Dense for transfer learning (`fine_tune_at`, `batchnorm`) - the
+native `ResNet50Engine(fine_tune_at=k)` on an H100 at a square size that is a multiple of 32, else `ResNet50Head`.
 """
 from __future__ import annotations
 
@@ -38,20 +40,41 @@ def build_model(img_height: int = IMG_HEIGHT, img_width: int = IMG_WIDTH, img_ch
 
     ``batchnorm`` (MobileNetV2 with ``fine_tune_at`` only): ``"inference"`` (default) as above, or ``"training"`` - the
     BatchNorms of ``base.features[k:]`` normalise with batch statistics in training steps and update their running
-    statistics; ``evaluate`` / ``predict`` use the running statistics."""
+    statistics; ``evaluate`` / ``predict`` use the running statistics.
+
+    ``arch="resnet50_head"`` is the same recipe with a ResNet-50 base: ``fine_tune_at=k`` in 0..17 (0 = stem, 1..16 =
+    bottleneck blocks ``layer1.0`` .. ``layer4.2``, 17 = head only; None means 17) and the same ``batchnorm`` modes.
+    It has no ``freeze_base=False``: the fully trainable model is ``arch="resnet50"``."""
     if isinstance(img_height, float) and img_width == IMG_WIDTH:  # build_model(dropout) positional form
         dropout, img_height = img_height, IMG_HEIGHT
     if img_channels != 3:
         raise ValueError("only 3-channel images are supported")
     augmentation = check_augmentation(augmentation)
-    from .mobilenet import check_batchnorm
+    from .mobilenet import check_batchnorm, check_fine_tune_at
 
     check_batchnorm(batchnorm, fine_tune_at)
+    if arch == "resnet50_head":
+        from .resnet_engine import NUM_FEATURE_BLOCKS
+
+        if not freeze_base:
+            raise ValueError("arch='resnet50_head' fine-tunes a frozen base; the fully trainable model is arch='resnet50'")
+        check_fine_tune_at(fine_tune_at, num_blocks=NUM_FEATURE_BLOCKS)
+        k = NUM_FEATURE_BLOCKS if fine_tune_at is None else fine_tune_at
+        if torch.cuda.is_available() and img_height == img_width and img_height % 32 == 0 \
+                and (device is None or torch.device(device).type == "cuda"):
+            from .resnet_engine import ResNet50Engine
+
+            return ResNet50Engine(batch=batch_size, num_classes=num_classes, device=device, image_size=img_height,
+                                  dropout=dropout, seed=seed, augmentation=augmentation, fine_tune_at=k,
+                                  batchnorm=batchnorm, **engine_kwargs)
+        from .resnet import ResNet50Head
+
+        with torch.random.fork_rng(devices=[]):
+            torch.manual_seed(seed)
+            return ResNet50Head(num_classes, dropout, k, batchnorm, augmentation=augmentation, augmentation_seed=seed)
     if batchnorm == "training" and arch in ("resnet50", "resnet50_torch"):
         raise ValueError("batchnorm='training' applies to the MobileNetV2 model only")
     if fine_tune_at is not None:
-        from .mobilenet import check_fine_tune_at
-
         check_fine_tune_at(fine_tune_at, freeze_base)
         if arch is None:
             arch = "mobilenetv2"

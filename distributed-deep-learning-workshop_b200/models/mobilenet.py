@@ -58,14 +58,16 @@ class MobileNetV2Base(nn.Module):
 NUM_FEATURE_BLOCKS = 19   # base.features: stem, 17 inverted-residual blocks, last 1x1 conv
 
 
-def check_fine_tune_at(fine_tune_at, freeze_base: bool = True) -> None:
+def check_fine_tune_at(fine_tune_at, freeze_base: bool = True, num_blocks: int = NUM_FEATURE_BLOCKS) -> None:
+    """``fine_tune_at`` is None or an int in 0..``num_blocks`` (the head-only value of the architecture: 19 for
+    MobileNetV2, 17 for ResNet-50)."""
     if fine_tune_at is None:
         return
     if not freeze_base:
         raise ValueError("fine_tune_at keeps the base's BatchNorm in inference mode; freeze_base=False trains it in "
                          "training mode - pass one or the other")
-    if isinstance(fine_tune_at, bool) or not isinstance(fine_tune_at, int) or not 0 <= fine_tune_at <= NUM_FEATURE_BLOCKS:
-        raise ValueError(f"fine_tune_at must be an int in 0..{NUM_FEATURE_BLOCKS}, got {fine_tune_at!r}")
+    if isinstance(fine_tune_at, bool) or not isinstance(fine_tune_at, int) or not 0 <= fine_tune_at <= num_blocks:
+        raise ValueError(f"fine_tune_at must be an int in 0..{num_blocks}, got {fine_tune_at!r}")
 
 
 BATCHNORM_MODES = ("inference", "training")

@@ -16,6 +16,16 @@ ready front-to-back and `DistributedOptimizer` can all-reduce bucket k while buc
 Conv filters use the kernel layout ``[R*S, Cout, Cin]``; `state_dict()` converts to torch's OIHW.
 
 Reference call sites this replaces: `build_model` (P1/03:159-178), `model.fit` inner step (P1/03:353-358).
+
+``fine_tune_at=k`` (``arch = "resnet50_head"``) trains only feature blocks ``k..16`` (0 = stem, 1..16 = the bottleneck
+blocks in order, 17 = the head alone) and the Dense head.  The frozen prefix runs the inference build's convolutions
+(folded BatchNorm + ReLU + residual in the epilogue, scale / shift from the running statistics refreshed by
+`sync_weights`), stores nothing for a backward pass, and the backward pass stops at block ``k``: its conv1 /
+downsample data gradients are never built.  Because the flat layout is in backward-completion order, the trainable
+tensors are the prefix ``params[:trainable_numel]`` and the gradient buffer, the optimizer and the all-reduce cover only
+it.  ``batchnorm="training"`` runs the trainable blocks exactly as the fully trainable engine does;
+``batchnorm="inference"`` normalises them with their running statistics (no statistics epilogue, never updated) and
+their backward uses bn_bwd_coeffs' inference mode (dy = gamma * invstd_run * dz).
 """
 from __future__ import annotations
 
@@ -102,6 +112,19 @@ def _kd_head(student, mix, dlogits16) -> None:
                                student.loss_rows, student.stats, 1.0 / N)
 
 
+NUM_FEATURE_BLOCKS = 17   # fine_tune_at: 0 = stem, 1..16 = bottleneck blocks, 17 = head only
+
+
+def feature_block(name: str) -> int:
+    """Feature block (``fine_tune_at`` numbering) of a torchvision ResNet-50 state-dict name."""
+    if name.startswith("fc."):
+        return NUM_FEATURE_BLOCKS
+    if name.startswith("layer"):
+        stage, idx = name.split(".")[:2]
+        return 1 + sum((3, 4, 6, 3)[:int(stage[5:]) - 1]) + int(idx)
+    return 0
+
+
 def resnet50_blocks(image_size: int = 224) -> List[BlockSpec]:
     cfg = [(64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)]
     blocks = []
@@ -126,12 +149,35 @@ class ResNet50Engine:
                  seed: int = 0, max_ctas: int = 0, zero_init_residual: bool = True, native_stem: bool = True,
                  overlap_wgrad: bool = True, wgrad_smem_budget: int = 0, fuse_bwd_reduce: bool = True,
                  fuse_bn_coeffs: bool = False, fuse_block_grad: Optional[bool] = None,
-                 fuse_stem_bwd: Optional[bool] = None, augmentation=None):
+                 fuse_stem_bwd: Optional[bool] = None, augmentation=None, fine_tune_at: Optional[int] = None,
+                 batchnorm: str = "inference"):
         """``augmentation`` (`models.augment.Augmentation`): random flip / rotation / zoom / translation of the input
-        batch in every training step, on the device (see `models.augment`); evaluation and inference never apply it."""
+        batch in every training step, on the device (see `models.augment`); evaluation and inference never apply it.
+
+        ``fine_tune_at=k`` (0..17): train feature blocks ``k..16`` and the head only (module doc); None (default) is the
+        fully trainable engine.  ``batchnorm`` (read only with ``fine_tune_at``): ``"inference"`` normalises every
+        BatchNorm with its running statistics, which never change; ``"training"`` gives the trainable blocks batch
+        statistics and the running-statistics update.  The in-kernel training-mode coefficient paths
+        (``fuse_bn_coeffs``, ``fuse_stem_bwd``) are refused with ``"inference"``, and their environment switches
+        (B200DDL_FUSE_BN_COEFFS, B200DDL_STEM_BWD_FUSE, B200DDL_TAILS) are ignored there."""
         from .augment import check_augmentation
+        from .mobilenet import check_batchnorm, check_fine_tune_at
 
         ops.require_native()
+        check_fine_tune_at(fine_tune_at, num_blocks=NUM_FEATURE_BLOCKS)
+        check_batchnorm(batchnorm, fine_tune_at)
+        self.fine_tune_at = fine_tune_at
+        self.batchnorm = batchnorm
+        # k: first trainable feature block (0 = stem ... 17 = head only); the fully trainable engine is k = 0 in training mode
+        self._k = 0 if fine_tune_at is None else fine_tune_at
+        self._first = max(self._k - 1, 0)   # index in `blocks` of the first trainable block (16: none)
+        # k = 17 has no trainable BatchNorm: both modes are the same engine
+        self._bn_train = fine_tune_at is None or (batchnorm == "training" and fine_tune_at < NUM_FEATURE_BLOCKS)
+        if fine_tune_at is not None:
+            self.arch = "resnet50_head"
+        if not self._bn_train and (fuse_bn_coeffs or fuse_stem_bwd):
+            raise ValueError("fuse_bn_coeffs / fuse_stem_bwd compute training-mode BatchNorm coefficients: they do not "
+                             "apply to batchnorm='inference'")
         self.augmentation = check_augmentation(augmentation)
         self._augmenter = None
         # Keras's label smoothing of the loss; the Trainer sets it from the compiled loss before capturing the steps
@@ -148,13 +194,14 @@ class ResNet50Engine:
         # OPT-IN (B200DDL_FUSE_BN_COEFFS=1): BatchNorm scale/shift (forward) and A/B/C (backward) computed inside the apply
         # kernels instead of 106 tiny launches.  Numerically equivalent (backward bit-identical); opt-in because the per-CTA
         # coefficient recomputation in 106 streaming kernels can cost more than the tiny dependent launches it replaces.
-        self.fuse_bn_coeffs = fuse_bn_coeffs or os.environ.get("B200DDL_FUSE_BN_COEFFS") == "1"
+        self.fuse_bn_coeffs = (fuse_bn_coeffs or os.environ.get("B200DDL_FUSE_BN_COEFFS") == "1") and self._bn_train
         # the gradient merge at every residual-block boundary (main path + skip path, ReLU mask, bn3 reduction) runs in
         # the epilogue of the next block's conv1 dgrad GEMM (conv_igemm kStats = 3); B200DDL_NO_BLOCK_GRAD=1 disables
         self.fuse_block_grad = (os.environ.get("B200DDL_NO_BLOCK_GRAD") != "1") if fuse_block_grad is None else bool(fuse_block_grad)
         # max-pool backward fused with the stem BatchNorm backward (csrc/head_stem.cu); B200DDL_STEM_BWD_FUSE=1 enables
         # (opt-in):
-        self.fuse_stem_bwd = (os.environ.get("B200DDL_STEM_BWD_FUSE") == "1") if fuse_stem_bwd is None else bool(fuse_stem_bwd)
+        self.fuse_stem_bwd = ((os.environ.get("B200DDL_STEM_BWD_FUSE") == "1") if fuse_stem_bwd is None
+                              else bool(fuse_stem_bwd)) and self._bn_train
         self._fused_reduce = set()
         self._block_fused = set()   # bn3 names whose reduction (and dz) come out of a fused dgrad epilogue
         # inference-only builds (build(training=False)): BatchNorm (running statistics) + ReLU + residual add run in the
@@ -165,7 +212,7 @@ class ResNet50Engine:
         # accumulated the sums (conv_igemm last-CTA tails) instead of ~100 tiny dependent launches per step.  Numerically
         # equivalent (gpu_check.py tails); opt-in because fence + ticket + a serial per-channel loop in ONE CTA at the end of
         # every GEMM can cost more than a tiny dependent kernel that runs on all SMs.
-        self.fuse_tails = os.environ.get("B200DDL_TAILS") == "1" and not self.fuse_bn_coeffs
+        self.fuse_tails = os.environ.get("B200DDL_TAILS") == "1" and not self.fuse_bn_coeffs and self._bn_train
         self._fin_fwd = set()    # BatchNorms finalized by their producing conv's tail (training mode)
         self._fin_bwd = set()    # BatchNorms whose backward coefficients come from a dgrad tail
         self._tail_plans = []
@@ -228,6 +275,10 @@ class ResNet50Engine:
         self.param_specs = specs
         self.spec = {s.name: s for s in specs}
         self.flat_numel = off
+        # fine-tuning: the trainable tensors (feature block >= k) are a prefix of the backward-completion layout
+        self.trainable_specs = [s for s in specs if feature_block(s.name) >= self._k]
+        assert self.trainable_specs == specs[:len(self.trainable_specs)]
+        self.trainable_numel = sum(_align(s.numel) for s in self.trainable_specs)
 
     def _alloc_params(self, seed: int) -> None:
         dev = self.device
@@ -282,16 +333,27 @@ class ResNet50Engine:
         """Refresh every bf16 working copy from the fp32 master (after an optimizer step or a weight load)."""
         self._e.cast_bf16(self.params, self.w16)
         if self._built:
+            if self._k > 0:
+                self._refresh_frozen()
             self.refresh_derived_weights()
 
     def refresh_derived_weights(self) -> None:
         """bf16 copies in layouts other than the master's: dgrad filters (one batched kernel + the few stride-2
-        tap subsets) and the packed stem filter."""
+        tap subsets) and the packed stem filter (a frozen stem's only changes with `sync_weights`)."""
         if getattr(self, "_wd_total", 0) > 0:
             self._e.weight_prep_batched(self.params, self._wd16, self._wd_table, self._wd_tiles)
-        self._refresh_stem_weight()
+        if self._k == 0:
+            self._refresh_stem_weight()
         if self._infer_fused:
             self._refresh_eval_affine()
+
+    def _refresh_frozen(self) -> None:
+        """Frozen prefix of a fine-tuning engine: the packed stem filter and the running-statistics scale / shift its
+        fused epilogues read.  Neither changes in a training step, so this runs at weight loads / syncs only."""
+        self._refresh_stem_weight()
+        for b in self.blocks[:self._first]:
+            for bn in ("bn1", "bn2", "bn3", "downsample.1") if b.downsample else ("bn1", "bn2", "bn3"):
+                self._bn_fwd(b.name + "." + bn, 1.0, False)
 
     def _refresh_eval_affine(self) -> None:
         """scale / shift of every BatchNorm from its running statistics (inference epilogues read them)."""
@@ -309,9 +371,10 @@ class ResNet50Engine:
 
     # ------------------------------------------------------------------------------------------------ build
     def bind_grad_buffer(self, grads: Optional[torch.Tensor] = None) -> None:
+        """Gradients of the trainable prefix ``params[:trainable_numel]`` (all of them without ``fine_tune_at``)."""
         if grads is None:
-            grads = torch.zeros(self.flat_numel, device=self.device, dtype=torch.float32)
-        assert grads.numel() >= self.flat_numel and grads.dtype == torch.float32
+            grads = torch.zeros(self.trainable_numel, device=self.device, dtype=torch.float32)
+        assert grads.numel() >= self.trainable_numel and grads.dtype == torch.float32
         self.grads = grads
 
     def build(self, training: bool = True) -> "ResNet50Engine":
@@ -376,6 +439,9 @@ class ResNet50Engine:
 
         max_act = N * (S // 4) * (S // 4) * 256
         max_act = max(max_act, N * H0 * H0 * 64)
+        if self._k > 0:   # the backward stops at block k: scratch for the largest trainable layer (none at k = 17)
+            max_act = max([N * b.h_in ** 2 * max(b.cin, b.mid) for b in self.blocks[self._first:]] +
+                          [N * b.h_out ** 2 * b.mid * 4 for b in self.blocks[self._first:]], default=0)
         if training:
             self._scr = {k: torch.zeros(max_act, **bf) for k in ("dy", "dyB", "da", "dds", "dzA", "dzB")}
             # the downsample branch runs between bn1's backward and conv1's (whose dy sits in "dy"): always its own buffer
@@ -416,11 +482,16 @@ class ResNet50Engine:
 
         fuse_bg = self.fuse_block_grad and training
         if training:
-            add_dgrad_weights("fc", [[0]])
+            if self._k < NUM_FEATURE_BLOCKS:
+                add_dgrad_weights("fc", [[0]])
             for bi, b in enumerate(self.blocks):
+                if bi < self._first:
+                    continue   # frozen prefix: no backward
                 for cname, k, stride in (("conv1", 1, 1), ("conv2", 3, b.stride), ("conv3", 1, 1),
                                          ("downsample.0", 1, b.stride)):
                     if cname == "downsample.0" and not b.downsample:
+                        continue
+                    if cname in ("conv1", "downsample.0") and not self._needs_dx(bi):
                         continue
                     if cname == "downsample.0" and stride == 2 and fuse_bg and bi > 0:
                         parts = [[0]]  # compact dgrad: a dense 1x1 GEMM on the strided grid
@@ -469,7 +540,9 @@ class ResNet50Engine:
             plan.set_bn_bwd_coeffs(next_counter(), self.p(bn_name + ".weight"), w_["mean"], w_["invstd"], float(count),
                                    self.g(bn_name + ".weight"), self.g(bn_name + ".bias"), w_["cA"], w_["cB"], w_["cC"])
             self._fin_bwd.add(bn_name)
-        for bi, b in enumerate(self.blocks if self._infer_fused else []):
+        # inference builds, and the frozen prefix of a fine-tuning engine
+        n_fused = len(self.blocks) if self._infer_fused else self._first
+        for bi, b in enumerate(self.blocks[:n_fused]):
             # inference: every convolution writes its block activation directly (folded BN + ReLU [+ residual] epilogue)
             Hi, Ho, mid, cout = b.h_in, b.h_out, b.mid, b.mid * 4
             A, n = self.act, b.name
@@ -497,7 +570,9 @@ class ResNet50Engine:
             self._fwd[n + ".conv3"] = C.ConvForward(A[n + ".a2"], w2d(n + ".conv3"), A[n + ".out"], 1, 1, 1, 0, None, None,
                                                     mc, epilogue=aff("bn3", "relu", res))
             x_in = A[n + ".out"]
-        for bi, b in enumerate([] if self._infer_fused else self.blocks):
+        for bi, b in enumerate(self.blocks):
+            if bi < n_fused:
+                continue
             Hi, Ho, mid, cout = b.h_in, b.h_out, b.mid, b.mid * 4
             A = self.act
             A[b.name + ".y1"] = torch.zeros(N, Hi, Hi, mid, **bf)
@@ -520,7 +595,9 @@ class ResNet50Engine:
                 w2d = w.view(w.shape[0] * w.shape[1], w.shape[2])
                 bw_ = self.bnw[b.name + "." + bnk]
                 y = A[b.name + "." + yk]
-                self._fwd[full] = C.ConvForward(xin, w2d, y, k, k, stride, pad, bw_["sum"], bw_["sqsum"], mc)
+                # running-statistics BatchNorm (batchnorm="inference") needs no batch statistics
+                st = (bw_["sum"], bw_["sqsum"]) if self._bn_train else (None, None)
+                self._fwd[full] = C.ConvForward(xin, w2d, y, k, k, stride, pad, *st, mc)
                 if training and self.fuse_tails:
                     bname = b.name + "." + bnk
                     cnt = N * y.shape[1] * y.shape[2]
@@ -535,6 +612,8 @@ class ResNet50Engine:
                     gw = self.g(full + ".weight")
                     self._wg[full] = C.ConvWgrad(dy, xin, gw.view(gw.shape[0] * gw.shape[1], gw.shape[2]), k, k,
                                                  stride, pad, 0, mc, self.wgrad_smem_budget)
+                    if cname in ("conv1", "downsample.0") and not self._needs_dx(bi):
+                        continue   # the first trainable block's input belongs to the frozen prefix: no data gradient
                     bwd_stats = None
                     block_grad = None
                     d_stride = stride
@@ -586,9 +665,10 @@ class ResNet50Engine:
             self.dpooled = torch.zeros(N, 2048, **bf)
             self._fc_wg = C.ConvWgrad(self.dlogits16.view(N, 1, 1, ncp), self.pooled.view(N, 1, 1, 2048),
                                       self.g("fc.weight"), 1, 1, 1, 0, 0, mc, 0)
-            self._fc_dg = C.ConvDgrad(self.dlogits16.view(N, 1, 1, ncp), self.p("fc.weight").view(1, ncp, 2048),
-                                      self.dpooled.view(N, 1, 1, 2048), 1, 1, 1, 0, mc, wbufs=wd_views("fc"))
-            if self.native_stem:
+            self._fc_dg = None if self._k == NUM_FEATURE_BLOCKS else \
+                C.ConvDgrad(self.dlogits16.view(N, 1, 1, ncp), self.p("fc.weight").view(1, ncp, 2048),
+                            self.dpooled.view(N, 1, 1, 2048), 1, 1, 1, 0, mc, wbufs=wd_views("fc"))
+            if self.native_stem and self._k == 0:
                 dy0 = self._scr["dzA"][:self.y0.numel()].view(self.y0.shape)
                 self._stem_wg = C.StemWgrad(x_train, dy0, self.g("conv1.weight").view(-1), max_ctas=self.max_ctas)
         self._training_built = training
@@ -597,6 +677,10 @@ class ResNet50Engine:
         if training and self.distillation is not None:
             self.distillation.teacher.bind_teacher_input(self._stem_input(True))
         return self
+
+    def _needs_dx(self, bi: int) -> bool:
+        """Whether block ``bi``'s input gradient is computed: not for the first trainable block above a frozen prefix."""
+        return bi >= self._k
 
     # ------------------------------------------------------------------------------------------------ forward
     def _bn_fwd(self, bn: str, count: float, training: bool) -> Dict[str, torch.Tensor]:
@@ -665,34 +749,37 @@ class ResNet50Engine:
             self.y0.copy_(y0.permute(0, 2, 3, 1))
             e.channel_stats(self.y0, w0["sum"], w0["sqsum"])
         cnt0 = N * self.y0.shape[1] * self.y0.shape[2]
-        self._bn_fwd("bn1", cnt0, training)
+        bn_train = training and self._bn_train   # trainable blocks' BatchNorms normalise with batch statistics
+        self._bn_fwd("bn1", cnt0, bn_train and self._k == 0)
         # BN + ReLU + 3x3/2 max-pool in one pass (the 112x112 activation is never written)
         e.bn_relu_maxpool_fwd(self.y0, w0["scale"], w0["shift"], self.p0, self.pool_idx)
         x_in = self.p0
-        if self._infer_fused and not training:
-            for b in self.blocks:
+        n_fused = len(self.blocks) if (self._infer_fused and not training) else self._first
+        if n_fused:
+            for b in self.blocks[:n_fused]:
                 n = b.name
                 self._fwd[n + ".conv1"].run()
                 self._fwd[n + ".conv2"].run()
                 if b.downsample:
                     self._fwd[n + ".downsample.0"].run()
                 self._fwd[n + ".conv3"].run()
-        for b in ([] if (self._infer_fused and not training) else self.blocks):
+            x_in = A[self.blocks[n_fused - 1].name + ".out"]
+        for b in self.blocks[n_fused:]:
             n = b.name
             cnt_in = N * b.h_in * b.h_in
             cnt_out = N * b.h_out * b.h_out
             self._fwd[n + ".conv1"].run()
-            self._bn_apply(n + ".bn1", cnt_in, training, A[n + ".y1"], A[n + ".a1"])
+            self._bn_apply(n + ".bn1", cnt_in, bn_train, A[n + ".y1"], A[n + ".a1"])
             self._fwd[n + ".conv2"].run()
-            self._bn_apply(n + ".bn2", cnt_out, training, A[n + ".y2"], A[n + ".a2"])
+            self._bn_apply(n + ".bn2", cnt_out, bn_train, A[n + ".y2"], A[n + ".a2"])
             self._fwd[n + ".conv3"].run()
             mask = A.get(n + ".mask") if training else None
             if b.downsample:
                 self._fwd[n + ".downsample.0"].run()
-                self._bn_apply(n + ".bn3", cnt_out, training, A[n + ".y3"], A[n + ".out"], A[n + ".yd"],
+                self._bn_apply(n + ".bn3", cnt_out, bn_train, A[n + ".y3"], A[n + ".out"], A[n + ".yd"],
                                n + ".downsample.1", mask)
             else:
-                self._bn_apply(n + ".bn3", cnt_out, training, A[n + ".y3"], A[n + ".out"], x_in, None, mask)
+                self._bn_apply(n + ".bn3", cnt_out, bn_train, A[n + ".y3"], A[n + ".out"], x_in, None, mask)
             x_in = A[n + ".out"]
         drop = self.dropout if training else 0.0
         self._drop_seed = self.seed * 1000003 + self._step_count
@@ -748,8 +835,10 @@ class ResNet50Engine:
                                  w["invstd"], float(count), self.g(bn + ".weight"), self.g(bn + ".bias"), dy)
         else:
             if bn not in self._fin_bwd:  # otherwise the dgrad GEMM's last CTA already produced dgamma / dbeta / A, B, C
+                # batchnorm="inference": mean / invstd are the running statistics and B = C = 0
                 e.bn_bwd_coeffs(w["sum_dz"], w["sum_dzy"], self.p(bn + ".weight"), w["mean"], w["invstd"], float(count),
-                                self.g(bn + ".weight"), self.g(bn + ".bias"), w["cA"], w["cB"], w["cC"])
+                                self.g(bn + ".weight"), self.g(bn + ".bias"), w["cA"], w["cB"], w["cC"],
+                                inference=not self._bn_train)
             e.bn_bwd_apply(src, y, sc, sh, w["cA"], w["cB"], w["cC"], dy)
         self._ready(bn + ".weight", bn + ".bias")
 
@@ -761,15 +850,19 @@ class ResNet50Engine:
         return self._scr[key][:int(math.prod(shape))].view(shape)
 
     def _conv_bwd(self, full: str, cname: str) -> None:
-        """dgrad on the compute stream; wgrad either in line or on the side stream once dgrad has been issued."""
+        """dgrad on the compute stream; wgrad either in line or on the side stream once dgrad has been issued.  The first
+        trainable block above a frozen prefix has no conv1 / downsample dgrad."""
+        dg = self._dg.get(full)
         if not self.overlap_wgrad:
             self._wg[full].run()
-            self._dg[full].run()
+            if dg is not None:
+                dg.run()
             # only after every reader of this layer's weights has been enqueued: with fused_update the bucket kernel
             # launched from the hook rewrites them
             self._ready(full + ".weight")
             return
-        self._dg[full].run()
+        if dg is not None:
+            dg.run()
         ev = torch.cuda.Event()
         ev.record()
         self._wg_stream.wait_event(ev)
@@ -789,6 +882,9 @@ class ResNet50Engine:
         # classifier head: wgrad + dgrad on the wgmma GEMMs, bias gradient = column sums of dlogits
         self._fc_wg.run()
         e.fc_bias_grad(self.dlogits16, self.g("fc.bias"))
+        if self._fc_dg is None:   # fine_tune_at=17: the head is all that trains
+            self._ready("fc.weight", "fc.bias")
+            return
         self._fc_dg.run()
         self._ready("fc.weight", "fc.bias")
         drop = self.dropout
@@ -797,7 +893,7 @@ class ResNet50Engine:
         e.gap_bwd(self.dpooled, g1, drop, self._drop_seed)
         g2 = None
         dz_keys = ["dzA", "dzB"]
-        for bi in range(len(self.blocks) - 1, -1, -1):
+        for bi in range(len(self.blocks) - 1, self._first - 1, -1):
             b = self.blocks[bi]
             n = b.name
             x_in = A[self.blocks[bi - 1].name + ".out"] if bi > 0 else self.p0
@@ -828,13 +924,21 @@ class ResNet50Engine:
                 dyd = self._dy_buf("downsample.0", yd.shape)
                 self._bn_bwd(n + ".downsample.1", 3, dz, None, None, yd, dyd, None, cnt_out)
                 self._conv_bwd(n + ".downsample.0", "downsample.0")  # dgrad -> dds (x_in-shaped, or compact)
-                g2 = self._dg[n + ".downsample.0"].dx
+                g2 = self._dg[n + ".downsample.0"].dx if self._needs_dx(bi) else None
             else:
                 g2 = dz
             # dgrad -> main-path gradient of the block input, or (fused) the previous block's complete dz
             self._conv_bwd(n + ".conv1", "conv1")
-            g1 = self._dg[n + ".conv1"].dx
-        # stem: g1 (main path of layer1.0) + g2 (its projection shortcut) flow through max-pool, ReLU and bn1
+            g1 = self._dg[n + ".conv1"].dx if self._needs_dx(bi) else None
+        if self._k == 0:
+            self._backward_stem(g1, g2)
+        if self.overlap_wgrad:
+            torch.cuda.current_stream().wait_stream(self._wg_stream)
+            self._dy_reader.clear()
+
+    def _backward_stem(self, g1, g2) -> None:
+        """stem: g1 (main path of layer1.0) + g2 (its projection shortcut) flow through max-pool, ReLU and bn1."""
+        e, N = self._e, self.batch
         dy0 = self._scr["dzA"][:self.y0.numel()].view(self.y0.shape)
         cnt0 = N * self.y0.shape[1] * self.y0.shape[2]
         w0 = self.bnw["bn1"]
@@ -858,9 +962,6 @@ class ResNet50Engine:
                                              stride=2, padding=3)
             self.g("conv1.weight").view(7, 7, 64, 3).copy_(gw.permute(2, 3, 0, 1))
         self._ready("conv1.weight")
-        if self.overlap_wgrad:
-            torch.cuda.current_stream().wait_stream(self._wg_stream)
-            self._dy_reader.clear()
 
     # ------------------------------------------------------------------------------------------------ utilities
     def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None) -> None:
@@ -947,6 +1048,10 @@ class ResNet50Engine:
     def num_parameters(self) -> int:
         return sum(s.numel for s in self.param_specs) - (self.classes_padded - self.num_classes) * 2048
 
+    def trainable_parameters(self) -> int:
+        """Unpadded count of the tensors the optimizer updates (all of them without ``fine_tune_at``)."""
+        return sum(s.numel for s in self.trainable_specs) - (self.classes_padded - self.num_classes) * 2048
+
 
 class EngineTrainStep:
     """forward + backward + (distributed) optimizer update of a `ResNet50Engine`, captured as ONE CUDA graph.
@@ -980,18 +1085,26 @@ class EngineTrainStep:
             optimizer.timeline = self.timeline
             optimizer.extra_wait_streams = engine.aux_streams if engine.aux_streams else []
         e = engine
-        ranges = [(s.offset, s.offset + _align(s.numel)) for s in e.param_specs]
+        # a fine-tuning engine's optimizer (state, accumulation, EMA, all-reduce buckets) covers its trainable prefix only
+        T = getattr(e, "trainable_numel", e.flat_numel)   # (the MobileNetV2 engine lays out trainable tensors only)
+        ranges = [(s.offset, s.offset + _align(s.numel)) for s in getattr(e, "trainable_specs", e.param_specs)]
+
+        def prefix(t):
+            return t if T == e.flat_numel else t[:T]
+
         if self._dist:
-            grads = optimizer.allocate_grads(e.flat_numel, e.device)
+            grads = optimizer.allocate_grads(T, e.device)
             e.bind_grad_buffer(grads)
+            if e.arch == "resnet50_head":
+                optimizer.fused_update = False   # its per-bucket kernels rewrite the symmetric copy of ALL weights
             if getattr(optimizer, "fused_update", False):
                 # fused all-reduce + SGD: master weights and the bf16 copy move to symmetric/multicast memory
                 e.params, e.w16 = optimizer.allocate_weights(e.params, e.w16)
-            optimizer.attach(e.params, ranges, e.w16, grads)
+            optimizer.attach(prefix(e.params), ranges, prefix(e.w16), grads)
             e.grad_hook = optimizer.on_grads_ready
         else:
             e.bind_grad_buffer()
-            optimizer.attach(e.params, e.grads, e.w16, segments=ranges)
+            optimizer.attach(prefix(e.params), e.grads, prefix(e.w16), segments=ranges)
         e.build(training=True)
         if self._dist:
             optimizer.extra_wait_streams = list(e.aux_streams)

@@ -19,12 +19,17 @@ def _describe(model) -> dict:
         desc = {"arch": getattr(model, "arch", "resnet50"), "num_classes": model.num_classes, "image_size": model.image_size,
                 "dropout": model.dropout, "batch": model.batch, "engine": True, "augmentation": _augmentation(model),
                 "seed": model.seed}   # the seed keys the augmentation draws: a reloaded engine continues the sequence
-        if desc["arch"] == "mobilenetv2":
+        if desc["arch"] in ("mobilenetv2", "resnet50_head"):
             desc["fine_tune_at"] = model.fine_tune_at
             desc["batchnorm"] = model.batchnorm
         return desc
     from ..models.mobilenet import FrozenBaseClassifier
+    from ..models.resnet import ResNet50Head
 
+    if isinstance(model, ResNet50Head):
+        return {"arch": "resnet50_head", "num_classes": model.fc.out_features, "dropout": model.dropout.p,
+                "fine_tune_at": model.fine_tune_at, "batchnorm": model.batchnorm, "augmentation": _augmentation(model),
+                "augmentation_seed": model.augmentation_seed}
     if isinstance(model, FrozenBaseClassifier):
         return {"arch": "mobilenetv2", "num_classes": model.fc.out_features, "dropout": model.dropout.p,
                 "freeze_base": model.freeze_base, "fine_tune_at": model.fine_tune_at, "batchnorm": model.batchnorm,
@@ -82,6 +87,19 @@ def load_model(model_uri: str, batch_size: Optional[int] = None, device=None):
         else:  # CPU box: same weights in the torchvision-architecture module (inference only: no augmentation)
             model = build_model(num_classes=desc["num_classes"], arch="resnet50_torch")
             model.load_state_dict(sd, strict=False)
+    elif desc["arch"] == "resnet50_head":   # the engine on a GPU, the torch module on a CPU (same state-dict keys)
+        gpu = desc.get("engine") and torch.cuda.is_available()
+        size = desc["image_size"] if gpu else 224
+        model = build_model(size, size, 3, desc["num_classes"], desc["dropout"], arch="resnet50_head",
+                            batch_size=batch_size or desc.get("batch", 32), device=device if gpu else "cpu",
+                            fine_tune_at=desc.get("fine_tune_at"), augmentation=aug,
+                            seed=desc.get("seed", desc.get("augmentation_seed", 0)),
+                            batchnorm=desc.get("batchnorm", "inference"))
+        if gpu:
+            model.load_state_dict(sd)
+        else:   # the engine keeps no num_batches_tracked
+            missing = model.load_state_dict(sd, strict=False).missing_keys
+            assert all(k.endswith("num_batches_tracked") for k in missing), missing
     elif desc.get("engine") and torch.cuda.is_available():  # saved from the native MobileNetV2 engine
         model = build_model(desc["image_size"], desc["image_size"], 3, desc["num_classes"], desc["dropout"],
                             arch="mobilenetv2", batch_size=batch_size or desc["batch"], device=device,
