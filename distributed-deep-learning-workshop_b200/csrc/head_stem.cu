@@ -37,20 +37,39 @@ __device__ __forceinline__ bf8 pack8h(const float (&f)[8]) {
 }
 __device__ __forceinline__ float bf16_round(float x) { return __bfloat162float(__float2bfloat16(x)); }
 
+// Per-row loss weight of the weighted head kernels (Keras's class_weight / sample_weight): the batch's row weight
+// rw[row] when rw is given, else the class table cw at the row's target class.  The unweighted instantiation is 1 and
+// weigh() returns its argument untouched, so those kernels compile to the unweighted code.  The weighted product is a
+// correctly rounded, uncontracted __fmul_rn: w = 1 gives the unweighted bits, a power of two scales them exactly.
+template <bool kWeighted>
+__device__ __forceinline__ float row_weight(const float* __restrict__ cw, const float* __restrict__ rw, int row,
+                                            int target) {
+  if (!kWeighted) return 1.f;
+  return rw != nullptr ? rw[row] : cw[target];
+}
+template <bool kWeighted>
+__device__ __forceinline__ float weigh(float v, float w) {
+  return kWeighted ? __fmul_rn(v, w) : v;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------ softmax CE head
 // One warp per row.  logit[k] = bf16 logits16[row, k] + bias[k] for k < K (row pitch ld >= K, padded columns ignored).
+// kWeighted: the row's loss, loss stat and dlogits are scaled by w = rw[row] (rw != nullptr) or cw[label]
+// (row_weight); the unweighted instantiation reads neither pointer.
+template <bool kWeighted>
 __global__ void softmax_ce_head_kernel(const __nv_bfloat16* __restrict__ logits16, int ld,
                                        const float* __restrict__ bias, const int64_t* __restrict__ labels,
                                        float* __restrict__ logits32, __nv_bfloat16* __restrict__ dlogits16,
                                        float* __restrict__ loss_rows, float* __restrict__ stats, int B, int K,
-                                       float grad_scale) {
+                                       float grad_scale, const float* __restrict__ cw, const float* __restrict__ rw) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= B) return;
   const __nv_bfloat16* row = logits16 + (int64_t)warp * ld;
   const int label = (int)labels[warp];
+  const float w = row_weight<kWeighted>(cw, rw, warp, label);
   float mx = -3.0e38f;
   int amax = 0;
   for (int k = lane; k < K; k += 32) {
@@ -74,24 +93,27 @@ __global__ void softmax_ce_head_kernel(const __nv_bfloat16* __restrict__ logits1
       float d = 0.f;
       if (k < K) {
         const float pk = __expf(__bfloat162float(row[k]) + bias[k] - mx) * inv;
-        d = (pk - (k == label ? 1.f : 0.f)) * grad_scale;
+        d = weigh<kWeighted>((pk - (k == label ? 1.f : 0.f)) * grad_scale, w);
       }
       drow[k] = __float2bfloat16(d);
     }
   }
   if (lane == 0) {
-    const float l = lse - (__bfloat162float(row[label]) + bias[label]);
+    const float l = weigh<kWeighted>(lse - (__bfloat162float(row[label]) + bias[label]), w);
     if (loss_rows != nullptr) loss_rows[warp] = l;
     atomicAdd(stats, l);
     atomicAdd(stats + 1, amax == label ? 1.f : 0.f);
   }
 }
 void softmax_ce_head(const void* logits16, int ld, const float* bias, const int64_t* labels, float* logits32,
-                     void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale, cudaStream_t s) {
+                     void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale, const float* cw,
+                     const float* rw, cudaStream_t s) {
   const int threads = 128;
   const int blocks = (B * 32 + threads - 1) / threads;
-  softmax_ce_head_kernel<<<blocks, threads, 0, s>>>((const __nv_bfloat16*)logits16, ld, bias, labels, logits32,
-                                                    (__nv_bfloat16*)dlogits16, loss_rows, stats, B, K, grad_scale);
+  const auto kernel = cw != nullptr || rw != nullptr ? softmax_ce_head_kernel<true> : softmax_ce_head_kernel<false>;
+  kernel<<<blocks, threads, 0, s>>>(
+    (const __nv_bfloat16*)logits16, ld, bias, labels, logits32, (__nv_bfloat16*)dlogits16, loss_rows, stats, B, K,
+    grad_scale, cw, rw);
 }
 
 // softmax_ce_head against a soft target, for MixUp / CutMix and label smoothing (eps):
@@ -104,11 +126,14 @@ void softmax_ce_head(const void* logits16, int ld, const float* bias, const int6
 // division (__fdiv_rn, also under --use_fast_math).  With mu = 0 and eps = 0 every product by lambda, 1 - eps, mu or
 // eps / K is by 1 or 0, so each output is bit for bit softmax_ce_head's.  That argmax is decided on the integers: y when
 // 2 num < den, y_partner when 2 num > den, the lower of the two on a tie.
+// kWeighted: the class table cw is read at that argmax (the row's target class).
+template <bool kWeighted>
 __global__ void softmax_ce_soft_head_kernel(const __nv_bfloat16* __restrict__ logits16, int ld,
                                             const float* __restrict__ bias, const int64_t* __restrict__ labels,
                                             const int4* __restrict__ mix, float eps, float* __restrict__ logits32,
                                             __nv_bfloat16* __restrict__ dlogits16, float* __restrict__ loss_rows,
-                                            float* __restrict__ stats, int B, int K, float grad_scale) {
+                                            float* __restrict__ stats, int B, int K, float grad_scale,
+                                            const float* __restrict__ cw, const float* __restrict__ rw) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= B) return;
@@ -125,6 +150,7 @@ __global__ void softmax_ce_soft_head_kernel(const __nv_bfloat16* __restrict__ lo
       target = twice < m1.w ? label : twice > m1.w ? plabel : min(label, plabel);
     }
   }
+  const float w = row_weight<kWeighted>(cw, rw, warp, target);
   const float lam = 1.f - mu, keep = 1.f - eps, epsk = __fdiv_rn(eps, (float)K);
   float mx = -3.0e38f;
   int amax = 0;
@@ -157,7 +183,7 @@ __global__ void softmax_ce_soft_head_kernel(const __nv_bfloat16* __restrict__ lo
       if (k < K) {
         const float pk = __expf(__bfloat162float(row[k]) + bias[k] - mx) * inv;
         const float tk = keep * ((k == label ? lam : 0.f) + (k == plabel ? mu : 0.f)) + epsk;
-        d = (pk - tk) * grad_scale;
+        d = weigh<kWeighted>((pk - tk) * grad_scale, w);
       }
       drow[k] = __float2bfloat16(d);
     }
@@ -165,7 +191,8 @@ __global__ void softmax_ce_soft_head_kernel(const __nv_bfloat16* __restrict__ lo
   if (lane == 0) {
     const float ly = __bfloat162float(row[label]) + bias[label];
     const float lp = __bfloat162float(row[plabel]) + bias[plabel];
-    const float l = keep * (lam * (lse - ly) + mu * (lse - lp)) + epsk * (sd + (float)K * (lse - mx));
+    const float l = weigh<kWeighted>(keep * (lam * (lse - ly) + mu * (lse - lp)) + epsk * (sd + (float)K * (lse - mx)),
+                                     w);
     if (loss_rows != nullptr) loss_rows[warp] = l;
     atomicAdd(stats, l);
     atomicAdd(stats + 1, amax == target ? 1.f : 0.f);
@@ -173,12 +200,14 @@ __global__ void softmax_ce_soft_head_kernel(const __nv_bfloat16* __restrict__ lo
 }
 void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const int64_t* labels, const int32_t* mix,
                           float eps, float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K,
-                          float grad_scale, cudaStream_t s) {
+                          float grad_scale, const float* cw, const float* rw, cudaStream_t s) {
   const int threads = 128;
   const int blocks = (B * 32 + threads - 1) / threads;
-  softmax_ce_soft_head_kernel<<<blocks, threads, 0, s>>>((const __nv_bfloat16*)logits16, ld, bias, labels,
-                                                         (const int4*)mix, eps, logits32, (__nv_bfloat16*)dlogits16,
-                                                         loss_rows, stats, B, K, grad_scale);
+  const auto kernel =
+      cw != nullptr || rw != nullptr ? softmax_ce_soft_head_kernel<true> : softmax_ce_soft_head_kernel<false>;
+  kernel<<<blocks, threads, 0, s>>>(
+    (const __nv_bfloat16*)logits16, ld, bias, labels, (const int4*)mix, eps, logits32, (__nv_bfloat16*)dlogits16,
+    loss_rows, stats, B, K, grad_scale, cw, rw);
 }
 
 // softmax_ce_soft_head plus knowledge distillation from a teacher's logits t (bf16 tlogits16 [B, tld] + tbias), at
@@ -191,13 +220,15 @@ void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const
 // 1 - alpha with correctly rounded, uncontracted operations: at alpha = 1 that is a product by 1 plus a product by 0, so
 // loss, dlogits and loss_rows are bit for bit softmax_ce_soft_head's (and softmax_ce_head's at eps = 0 without mix
 // rows).  The teacher's row is only read: its max, then exp((t - tmax) / T) twice.
+// kWeighted: as softmax_ce_soft_head's, with the two term stats weighted too.
+template <bool kWeighted>
 __global__ void softmax_kd_head_kernel(const __nv_bfloat16* __restrict__ logits16, int ld,
                                        const float* __restrict__ bias, const __nv_bfloat16* __restrict__ tlogits16,
                                        int tld, const float* __restrict__ tbias, const int64_t* __restrict__ labels,
                                        const int4* __restrict__ mix, float eps, float alpha, float T,
                                        float* __restrict__ logits32, __nv_bfloat16* __restrict__ dlogits16,
                                        float* __restrict__ loss_rows, float* __restrict__ stats, int B, int K,
-                                       float grad_scale) {
+                                       float grad_scale, const float* __restrict__ cw, const float* __restrict__ rw) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= B) return;
@@ -215,6 +246,7 @@ __global__ void softmax_kd_head_kernel(const __nv_bfloat16* __restrict__ logits1
       target = twice < m1.w ? label : twice > m1.w ? plabel : min(label, plabel);
     }
   }
+  const float w = row_weight<kWeighted>(cw, rw, warp, target);
   const float lam = 1.f - mu, keep = 1.f - eps, epsk = __fdiv_rn(eps, (float)K);
   const float beta = 1.f - alpha, invT = __fdiv_rn(1.f, T);
   float mx = -3.0e38f, tmx = -3.0e38f;
@@ -265,7 +297,7 @@ __global__ void softmax_kd_head_kernel(const __nv_bfloat16* __restrict__ logits1
         const float tk = keep * ((k == label ? lam : 0.f) + (k == plabel ? mu : 0.f)) + epsk;
         const float qk = __expf(zs) * invS;
         const float ds = (pk - tk) * grad_scale;   // softmax_ce_soft_head's dlogit
-        d = __fadd_rn(__fmul_rn(alpha, ds), __fmul_rn(beta, T * (qk - rk) * grad_scale));
+        d = weigh<kWeighted>(__fadd_rn(__fmul_rn(alpha, ds), __fmul_rn(beta, T * (qk - rk) * grad_scale)), w);
       }
     }
     if (drow != nullptr) drow[k] = __float2bfloat16(d);
@@ -276,24 +308,25 @@ __global__ void softmax_kd_head_kernel(const __nv_bfloat16* __restrict__ logits1
     const float lp = __bfloat162float(row[plabel]) + bias[plabel];
     const float ce = keep * (lam * (lse - ly) + mu * (lse - lp)) + epsk * (sd + (float)K * (lse - mx));
     const float kd = T * T * kl;
-    const float l = __fadd_rn(__fmul_rn(alpha, ce), __fmul_rn(beta, kd));   // no contraction: alpha = 1 gives ce
+    // no contraction: alpha = 1 gives ce
+    const float l = weigh<kWeighted>(__fadd_rn(__fmul_rn(alpha, ce), __fmul_rn(beta, kd)), w);
     if (loss_rows != nullptr) loss_rows[warp] = l;
     atomicAdd(stats, l);
     atomicAdd(stats + 1, amax == target ? 1.f : 0.f);
-    atomicAdd(stats + 2, ce);
-    atomicAdd(stats + 3, kd);
+    atomicAdd(stats + 2, weigh<kWeighted>(ce, w));
+    atomicAdd(stats + 3, weigh<kWeighted>(kd, w));
   }
 }
 void softmax_kd_head(const void* logits16, int ld, const float* bias, const void* tlogits16, int tld,
                      const float* tbias, const int64_t* labels, const int32_t* mix, float eps, float alpha, float T,
                      float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale,
-                     cudaStream_t s) {
+                     const float* cw, const float* rw, cudaStream_t s) {
   const int threads = 128;
   const int blocks = (B * 32 + threads - 1) / threads;
-  softmax_kd_head_kernel<<<blocks, threads, 0, s>>>((const __nv_bfloat16*)logits16, ld, bias,
-                                                    (const __nv_bfloat16*)tlogits16, tld, tbias, labels,
-                                                    (const int4*)mix, eps, alpha, T, logits32,
-                                                    (__nv_bfloat16*)dlogits16, loss_rows, stats, B, K, grad_scale);
+  const auto kernel = cw != nullptr || rw != nullptr ? softmax_kd_head_kernel<true> : softmax_kd_head_kernel<false>;
+  kernel<<<blocks, threads, 0, s>>>(
+    (const __nv_bfloat16*)logits16, ld, bias, (const __nv_bfloat16*)tlogits16, tld, tbias, labels, (const int4*)mix,
+    eps, alpha, T, logits32, (__nv_bfloat16*)dlogits16, loss_rows, stats, B, K, grad_scale, cw, rw);
 }
 
 // dbias[k] = sum_b dlogits16[b, k]   (thread per column: coalesced across k for every row)

@@ -59,8 +59,12 @@ void gap_fwd(const void* x, void* out, int N, int HW, int C, float drop_p, uint6
 void gap_bwd(const void* dout, void* dx, int N, int HW, int C, float drop_p, uint64_t seed, cudaStream_t s);
 void softmax_ce(const float* logits, const int64_t* labels, float* dlogits, float* loss_rows, float* stats, int B,
                 int K, float grad_scale, cudaStream_t s);
+// The three heads take an optional per-row loss weight (Keras class_weight / sample_weight): cw = fp32 [K] class table
+// read at the row's target class, or rw = fp32 [B] row weights, at most one of them; both nullptr launch the unweighted
+// kernel.  Weighted: loss_rows, the loss stat(s) and dlogits are scaled by the row's weight; the correct count is not.
 void softmax_ce_head(const void* logits16, int ld, const float* bias, const int64_t* labels, float* logits32,
-                     void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale, cudaStream_t s);
+                     void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale, const float* cw,
+                     const float* rw, cudaStream_t s);
 void fc_bias_grad(const void* dlogits16, int ld, float* dbias, int B, int K, cudaStream_t s);
 void pack_stem_weight(const float* w, void* out, cudaStream_t s);
 void stem_pool_bn_bwd(int pass, const void* idx, const void* g1, const void* g2, const void* y, const float* scale,
@@ -182,12 +186,12 @@ int augment_color(const uint8_t* src, uint8_t* dst, const int32_t* step, int N, 
 // nullptr (mu = 0: label smoothing alone)
 void softmax_ce_soft_head(const void* logits16, int ld, const float* bias, const int64_t* labels, const int32_t* mix,
                           float eps, float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K,
-                          float grad_scale, cudaStream_t s);
+                          float grad_scale, const float* cw, const float* rw, cudaStream_t s);
 // softmax_ce_soft_head's loss at weight alpha plus (1 - alpha) T^2 KL(softmax(t / T) || softmax(s / T)), t = the
 // teacher's bf16 logits [B, tld] + tbias; stats = [sum loss, correct, sum soft-target loss, sum T^2 KL]
 void softmax_kd_head(const void* logits16, int ld, const float* bias, const void* tlogits16, int tld,
                      const float* tbias, const int64_t* labels, const int32_t* mix, float eps, float alpha, float T,
                      float* logits32, void* dlogits16, float* loss_rows, float* stats, int B, int K, float grad_scale,
-                     cudaStream_t s);
+                     const float* cw, const float* rw, cudaStream_t s);
 
 }  // namespace b200

@@ -288,28 +288,44 @@ void softmax_ce(Tensor logits, Tensor labels, OptT dlogits, OptT loss_rows, Tens
                    (int)logits.size(0), (int)logits.size(1), (float)grad_scale, cur());
   after();
 }
+// Optional per-row loss weights of the three heads: class_weight fp32 [K] (read at the row's target class) or
+// row_weight fp32 [B], at most one; neither launches the unweighted kernel.
+static void head_weights(const OptT& class_weight, const OptT& row_weight, const Tensor& logits16, int64_t B,
+                         int64_t K) {
+  TORCH_CHECK(!(class_weight.has_value() && row_weight.has_value()), "pass class_weight or row_weight, not both");
+  if (class_weight.has_value()) {
+    vec(*class_weight, at::kFloat, K, "class_weight", 4);
+    TORCH_CHECK(class_weight->device() == logits16.device(), "class_weight must be on the device of logits16");
+  }
+  if (row_weight.has_value()) {
+    vec(*row_weight, at::kFloat, B, "row_weight", 4);
+    TORCH_CHECK(row_weight->device() == logits16.device(), "row_weight must be on the device of logits16");
+  }
+}
 // classifier head: bf16 logits [B, ld] (first K columns real) + fp32 bias -> loss / accuracy / bf16 dlogits [B, ld]
 void softmax_ce_head(Tensor logits16, Tensor bias, Tensor labels, OptT logits32, OptT dlogits16, OptT loss_rows,
-                     Tensor stats, double grad_scale) {
+                     Tensor stats, double grad_scale, OptT class_weight, OptT row_weight) {
   chk(logits16, at::kBFloat16, "logits16");
   chk(bias, at::kFloat, "bias");
   chk(labels, at::kLong, "labels");
   chk(stats, at::kFloat, "stats");
   TORCH_CHECK(logits16.dim() == 2 && bias.numel() <= logits16.size(1) && labels.numel() == logits16.size(0));
   const int B = (int)logits16.size(0), ld = (int)logits16.size(1), K = (int)bias.numel();
+  head_weights(class_weight, row_weight, logits16, B, K);
   if (logits32.has_value()) { chk(*logits32, at::kFloat, "logits32"); TORCH_CHECK(logits32->numel() == (int64_t)B * K); }
   if (dlogits16.has_value()) { chk(*dlogits16, at::kBFloat16, "dlogits16"); TORCH_CHECK(dlogits16->numel() == logits16.numel()); }
   b200::softmax_ce_head(logits16.data_ptr(), ld, bias.data_ptr<float>(), labels.data_ptr<int64_t>(),
                         logits32.has_value() ? logits32->data_ptr<float>() : nullptr,
                         dlogits16.has_value() ? dlogits16->data_ptr() : nullptr,
                         loss_rows.has_value() ? loss_rows->data_ptr<float>() : nullptr, stats.data_ptr<float>(), B, K,
-                        (float)grad_scale, cur());
+                        (float)grad_scale, fp(class_weight), fp(row_weight), cur());
   after();
 }
 // softmax_ce_head against the soft target of label smoothing `eps` and, with `mix` (int32 [B, 8] mix rows of
 // augment_mix_params), the partner's label at weight num / den; see csrc/head_stem.cu
 void softmax_ce_soft_head(Tensor logits16, Tensor bias, Tensor labels, OptT mix, double eps, OptT logits32,
-                          OptT dlogits16, OptT loss_rows, Tensor stats, double grad_scale) {
+                          OptT dlogits16, OptT loss_rows, Tensor stats, double grad_scale, OptT class_weight,
+                          OptT row_weight) {
   chk(logits16, at::kBFloat16, "logits16");
   chk(bias, at::kFloat, "bias");
   chk(labels, at::kLong, "labels");
@@ -322,6 +338,7 @@ void softmax_ce_soft_head(Tensor logits16, Tensor bias, Tensor labels, OptT mix,
   const int B = (int)logits16.size(0), ld = (int)logits16.size(1), K = (int)bias.numel();
   for (const Tensor* t : {&bias, &labels, &stats})
     TORCH_CHECK(t->device() == logits16.device(), "bias, labels and stats must be on the device of logits16");
+  head_weights(class_weight, row_weight, logits16, B, K);
   if (mix.has_value()) {
     chk(*mix, at::kInt, "mix");
     TORCH_CHECK(mix->dim() == 2 && mix->size(0) == B && mix->size(1) == b200::kAugMixFields,
@@ -349,14 +366,14 @@ void softmax_ce_soft_head(Tensor logits16, Tensor bias, Tensor labels, OptT mix,
                              logits32.has_value() ? logits32->data_ptr<float>() : nullptr,
                              dlogits16.has_value() ? dlogits16->data_ptr() : nullptr,
                              loss_rows.has_value() ? loss_rows->data_ptr<float>() : nullptr, stats.data_ptr<float>(), B,
-                             K, (float)grad_scale, cur());
+                             K, (float)grad_scale, fp(class_weight), fp(row_weight), cur());
   after();
 }
 // softmax_ce_soft_head plus distillation from the teacher's bf16 logits [B, tld] + tbias (tld >= K = bias.numel()) at
 // weight 1 - alpha and temperature T; stats: [sum loss, correct, sum student loss, sum distillation loss]
 void softmax_kd_head(Tensor logits16, Tensor bias, Tensor tlogits16, Tensor tbias, Tensor labels, OptT mix, double eps,
                      double alpha, double temperature, OptT logits32, OptT dlogits16, OptT loss_rows, Tensor stats,
-                     double grad_scale) {
+                     double grad_scale, OptT class_weight, OptT row_weight) {
   chk(logits16, at::kBFloat16, "logits16");
   chk(bias, at::kFloat, "bias");
   chk(tlogits16, at::kBFloat16, "tlogits16");
@@ -377,6 +394,7 @@ void softmax_kd_head(Tensor logits16, Tensor bias, Tensor tlogits16, Tensor tbia
   for (const Tensor* t : {&bias, &tlogits16, &tbias, &labels, &stats})
     TORCH_CHECK(t->device() == logits16.device(), "bias, the teacher's tensors, labels and stats must be on the device "
                 "of logits16");
+  head_weights(class_weight, row_weight, logits16, B, K);
   if (mix.has_value()) {
     chk(*mix, at::kInt, "mix");
     TORCH_CHECK(mix->dim() == 2 && mix->size(0) == B && mix->size(1) == b200::kAugMixFields,
@@ -406,7 +424,7 @@ void softmax_kd_head(Tensor logits16, Tensor bias, Tensor tlogits16, Tensor tbia
                         (float)temperature, logits32.has_value() ? logits32->data_ptr<float>() : nullptr,
                         dlogits16.has_value() ? dlogits16->data_ptr() : nullptr,
                         loss_rows.has_value() ? loss_rows->data_ptr<float>() : nullptr, stats.data_ptr<float>(), B, K,
-                        (float)grad_scale, cur());
+                        (float)grad_scale, fp(class_weight), fp(row_weight), cur());
   after();
 }
 void fc_bias_grad(Tensor dlogits16, Tensor dbias) {
@@ -966,16 +984,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("softmax_ce", &softmax_ce);
   m.def("softmax_ce_head", &softmax_ce_head, py::arg("logits16"), py::arg("bias"), py::arg("labels"),
         py::arg("logits32") = c10::nullopt, py::arg("dlogits16") = c10::nullopt, py::arg("loss_rows") = c10::nullopt,
-        py::arg("stats"), py::arg("grad_scale") = 1.0);
+        py::arg("stats"), py::arg("grad_scale") = 1.0,
+        py::arg("class_weight") = c10::nullopt, py::arg("row_weight") = c10::nullopt);
   m.def("softmax_ce_soft_head", &softmax_ce_soft_head, py::arg("logits16"), py::arg("bias"), py::arg("labels"),
         py::arg("mix") = c10::nullopt, py::arg("label_smoothing") = 0.0, py::arg("logits32") = c10::nullopt,
         py::arg("dlogits16") = c10::nullopt, py::arg("loss_rows") = c10::nullopt, py::arg("stats"),
-        py::arg("grad_scale") = 1.0);
+        py::arg("grad_scale") = 1.0,
+        py::arg("class_weight") = c10::nullopt, py::arg("row_weight") = c10::nullopt);
   m.def("softmax_kd_head", &softmax_kd_head, py::arg("logits16"), py::arg("bias"), py::arg("tlogits16"),
         py::arg("tbias"), py::arg("labels"), py::arg("mix") = c10::nullopt, py::arg("label_smoothing") = 0.0,
         py::arg("alpha") = 0.1, py::arg("temperature") = 3.0, py::arg("logits32") = c10::nullopt,
         py::arg("dlogits16") = c10::nullopt, py::arg("loss_rows") = c10::nullopt, py::arg("stats"),
-        py::arg("grad_scale") = 1.0);
+        py::arg("grad_scale") = 1.0,
+        py::arg("class_weight") = c10::nullopt, py::arg("row_weight") = c10::nullopt);
   m.def("fc_bias_grad", &fc_bias_grad);
   m.def("pack_stem_weight", &pack_stem_weight);
   m.def("stem_pool_bn_bwd", &stem_pool_bn_bwd, py::arg("pass_"), py::arg("idx"), py::arg("g1"), py::arg("g2"), py::arg("y"),

@@ -595,12 +595,20 @@ class Converter:
 
 class InMemoryDataset:
     """`toPandas()` + `from_tensor_slices((content, label_idx)).map(preprocess).batch(B)` (reference P1/02:97-139,
-    P2/01:137-151): the whole table is decoded once into driver memory; finite, re-iterable, `len()` = batches."""
+    P2/01:137-151): the whole table is decoded once into driver memory; finite, re-iterable, `len()` = batches.
+    ``weight_column``: batches are ``(images, labels, sample_weight float32 [B])`` with the weights read from that column
+    (Keras's ``(x, y, sample_weight)`` datasets)."""
 
-    def __init__(self, table_or_pdf, batch_size: int, image_size=(IMG_HEIGHT, IMG_WIDTH), drop_last: bool = True):
+    def __init__(self, table_or_pdf, batch_size: int, image_size=(IMG_HEIGHT, IMG_WIDTH), drop_last: bool = True,
+                 weight_column: Optional[str] = None):
         pdf = table_or_pdf.to_pandas() if hasattr(table_or_pdf, "to_pandas") else table_or_pdf
         self.images = torch.from_numpy(np.stack([decode_image(c, image_size) for c in pdf["content"]]))
         self.labels = torch.from_numpy(pdf["label_idx"].to_numpy(dtype=np.int64))
+        self.weights = None
+        if weight_column is not None:
+            if weight_column not in pdf.columns:
+                raise ValueError(f"weight_column {weight_column!r} is not a column of the table")
+            self.weights = torch.from_numpy(pdf[weight_column].to_numpy(dtype=np.float32))
         self.batch_size = max(1, min(batch_size, len(self.labels)))
         n = len(self.labels)
         self.n = n // self.batch_size * self.batch_size if drop_last else n
@@ -610,7 +618,11 @@ class InMemoryDataset:
 
     def __iter__(self):
         for i in range(0, self.n, self.batch_size):
-            yield self.images[i:i + self.batch_size], self.labels[i:i + self.batch_size]
+            if self.weights is None:
+                yield self.images[i:i + self.batch_size], self.labels[i:i + self.batch_size]
+            else:
+                yield (self.images[i:i + self.batch_size], self.labels[i:i + self.batch_size],
+                       self.weights[i:i + self.batch_size])
 
 
 def make_converter(table, cache_dir: Optional[str] = None) -> Converter:

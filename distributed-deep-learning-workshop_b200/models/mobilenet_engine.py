@@ -44,7 +44,8 @@ import torch
 
 from .. import ops
 from ..ops import conv as C
-from .resnet_engine import ParamSpec, _align, _augmenter, _kd_head, _stats_len, set_distillation
+from .resnet_engine import (ParamSpec, _align, _augmenter, _head_weights, _kd_head, _set_row_weight, _stats_len,
+                            set_class_weight, set_distillation, set_weighting)
 
 _CFG = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2), (6, 320, 1, 1)]
 
@@ -78,6 +79,10 @@ class MobileNetV2Engine:
         self.label_smoothing = 0.0
         self.distillation = None   # `train.losses.Distillation` with an engine teacher: set by `set_distillation`
         self._teacher_in: Optional[torch.Tensor] = None   # a student's stem input this engine reads as a teacher
+        # per-row loss weights of the training / evaluation head (`resnet_engine.set_weighting`) and their buffers
+        self.train_weighting = self.eval_weighting = None
+        self.class_weight: Optional[torch.Tensor] = None
+        self.row_weight: Optional[torch.Tensor] = None
         if image_size % 32:
             raise ValueError("image_size must be a multiple of 32")
         check_fine_tune_at(fine_tune_at)
@@ -571,14 +576,15 @@ class MobileNetV2Engine:
         e.zero_(self.stats)
         dl = self.dlogits16 if (training and self._training_built) else None
         mix = self._augmenter.mix if (training and self._augmenter is not None) else None
+        wts = _head_weights(self, training)
         if training and self.distillation is not None:
-            _kd_head(self, mix, dl)
+            _kd_head(self, mix, dl, wts)
         elif mix is None and self.label_smoothing == 0:
             e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits, dl, self.loss_rows,
-                              self.stats, 1.0 / N)
+                              self.stats, 1.0 / N, *wts)
         else:   # soft targets: the partner's label at the mix row's weight, label smoothing
             e.softmax_ce_soft_head(self.logits16, self.p("fc.bias"), self.labels, mix, self.label_smoothing,
-                                   self.logits, dl, self.loss_rows, self.stats, 1.0 / N)
+                                   self.logits, dl, self.loss_rows, self.stats, 1.0 / N, *wts)
 
     def backward(self) -> None:
         """Dense head weight / bias gradients; with fine_tune_at <= 18 also those of base.features[fine_tune_at:]."""
@@ -641,10 +647,21 @@ class MobileNetV2Engine:
         self._teacher_in = x_u8
         self.build(training=self.grads is not None)
 
-    def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None) -> None:
+    def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None,
+                  sample_weight: Optional[torch.Tensor] = None) -> None:
         self.x_u8.copy_(x_u8.view(self.x_u8.shape), non_blocking=True)
         if labels is not None:
             self.labels.copy_(labels, non_blocking=True)
+        if sample_weight is not None:
+            _set_row_weight(self, sample_weight)
+
+    def set_weighting(self, mode: Optional[str], training: bool = True) -> bool:
+        """Per-row loss weights of the training or evaluation head (see `resnet_engine.set_weighting`)."""
+        return set_weighting(self, mode, training)
+
+    def set_class_weight(self, table: torch.Tensor) -> None:
+        """New values of the class-weight table (float [K]); no graph needs capturing again."""
+        set_class_weight(self, table)
 
     def loss_and_acc(self) -> Tuple[float, float]:
         s = self.stats.tolist()

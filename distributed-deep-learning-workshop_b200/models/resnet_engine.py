@@ -103,13 +103,60 @@ def set_distillation(student, distillation) -> None:
         student.stats = torch.zeros(_stats_len(student), device=student.device, dtype=torch.float32)
 
 
-def _kd_head(student, mix, dlogits16) -> None:
+def _kd_head(student, mix, dlogits16, weights=(None, None)) -> None:
     """softmax_kd_head of a distilling student's logits16 against its teacher's (same batch row for row)."""
     d, N = student.distillation, student.batch
     t = d.teacher
     student._e.softmax_kd_head(student.logits16, student.p("fc.bias"), t.logits16, t.p("fc.bias"), student.labels, mix,
                                student.label_smoothing, d.alpha, d.temperature, student.logits, dlogits16,
-                               student.loss_rows, student.stats, 1.0 / N)
+                               student.loss_rows, student.stats, 1.0 / N, *weights)
+
+
+WEIGHTING_MODES = (None, "class", "sample")
+
+
+def set_weighting(engine, mode: Optional[str], training: bool = True) -> bool:
+    """Weight the per-row losses of either native engine's training (``training=True``) or evaluation head:
+    None (unweighted), ``"class"`` (Keras ``class_weight``: the table ``engine.class_weight`` [K] at each row's target
+    class; training only) or ``"sample"`` (the batch's ``sample_weight``: ``engine.row_weight`` [B], written by
+    ``set_input``).  The head kernel is chosen when a step is launched or captured, so the mode is part of a captured
+    graph; the two buffers are allocated on first use and never move, so new table or row values need no re-capture.
+    Returns whether the mode changed: graphs captured under the old mode must then be captured again."""
+    if mode not in WEIGHTING_MODES or (mode == "class" and not training):
+        raise ValueError(f"weighting mode must be one of {WEIGHTING_MODES} ('class' for training only), got {mode!r}")
+    if mode == "class":
+        _weight_buffer(engine, "class_weight", engine.num_classes)
+    elif mode == "sample":
+        _weight_buffer(engine, "row_weight", engine.batch)
+    attr = "train_weighting" if training else "eval_weighting"
+    changed = getattr(engine, attr) != mode
+    setattr(engine, attr, mode)
+    return changed
+
+
+def set_class_weight(engine, table: torch.Tensor) -> None:
+    """Copy a class-weight table (float [K]) into the engine's static table (asynchronously, like the labels)."""
+    _weight_buffer(engine, "class_weight", engine.num_classes).copy_(table.view(-1), non_blocking=True)
+
+
+def _weight_buffer(engine, name: str, n: int) -> torch.Tensor:
+    buf = getattr(engine, name)
+    if buf is None:
+        buf = torch.ones(n, device=engine.device, dtype=torch.float32)
+        setattr(engine, name, buf)
+    return buf
+
+
+def _set_row_weight(engine, w: torch.Tensor) -> None:
+    if w.numel() != engine.batch:
+        raise ValueError(f"sample_weight must hold one weight per row ({engine.batch}), got {tuple(w.shape)}")
+    _weight_buffer(engine, "row_weight", engine.batch).copy_(w.view(-1), non_blocking=True)
+
+
+def _head_weights(engine, training: bool):
+    """(class_weight, row_weight) arguments of the head kernels for the engine's weighting mode (at most one set)."""
+    mode = engine.train_weighting if training else engine.eval_weighting
+    return (engine.class_weight if mode == "class" else None, engine.row_weight if mode == "sample" else None)
 
 
 NUM_FEATURE_BLOCKS = 17   # fine_tune_at: 0 = stem, 1..16 = bottleneck blocks, 17 = head only
@@ -184,6 +231,10 @@ class ResNet50Engine:
         self.label_smoothing = 0.0
         self.distillation = None   # `train.losses.Distillation` with an engine teacher: set by `set_distillation`
         self._teacher_in: Optional[torch.Tensor] = None   # a student's stem input this engine reads as a teacher
+        # per-row loss weights of the training / evaluation head (`set_weighting`) and their buffers (allocated on use)
+        self.train_weighting = self.eval_weighting = None
+        self.class_weight: Optional[torch.Tensor] = None
+        self.row_weight: Optional[torch.Tensor] = None
         self.zero_init_residual = zero_init_residual
         self.native_stem = native_stem
         # experimental: run every weight-gradient GEMM on a side stream so it overlaps the (DRAM-bound) BatchNorm
@@ -788,19 +839,21 @@ class ResNet50Engine:
 
     def forward_head(self, training: bool = True) -> None:
         """+ bias, softmax cross-entropy, accuracy, bf16 dlogits (padded columns zero) in one kernel; against the soft
-        target when the batch is mixed or the labels smoothed, plus the teacher's term when distilling."""
+        target when the batch is mixed or the labels smoothed, plus the teacher's term when distilling; each row's loss
+        and dlogits weighted by its class or sample weight in a weighting mode (`set_weighting`)."""
         e, N = self._e, self.batch
         e.zero_(self.stats)
         mix = self._augmenter.mix if (training and self._augmenter is not None) else None
         dl = self.dlogits16 if training else None
+        wts = _head_weights(self, training)
         if training and self.distillation is not None:
-            _kd_head(self, mix, dl)
+            _kd_head(self, mix, dl, wts)
         elif mix is None and self.label_smoothing == 0:
             e.softmax_ce_head(self.logits16, self.p("fc.bias"), self.labels, self.logits, dl, self.loss_rows,
-                              self.stats, 1.0 / N)
+                              self.stats, 1.0 / N, *wts)
         else:   # soft targets: the partner's label at the mix row's weight, label smoothing
             e.softmax_ce_soft_head(self.logits16, self.p("fc.bias"), self.labels, mix, self.label_smoothing,
-                                   self.logits, dl, self.loss_rows, self.stats, 1.0 / N)
+                                   self.logits, dl, self.loss_rows, self.stats, 1.0 / N, *wts)
 
     # ------------------------------------------------------------------------------------------------ backward
     def _ready(self, *names: str) -> None:
@@ -964,10 +1017,12 @@ class ResNet50Engine:
         self._ready("conv1.weight")
 
     # ------------------------------------------------------------------------------------------------ utilities
-    def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None) -> None:
+    def set_input(self, x_u8: torch.Tensor, labels: Optional[torch.Tensor] = None,
+                  sample_weight: Optional[torch.Tensor] = None) -> None:
         """Copy a batch into the static input buffers.  Images whose spatial size differs from the engine's are resized
         ON THE GPU (bilinear, half-pixel centres like `tf.image.resize` - the reference's preprocess, P1/03:182-189):
-        the batch goes to a device staging buffer of its own size and `resize_bilinear_u8` writes the engine input."""
+        the batch goes to a device staging buffer of its own size and `resize_bilinear_u8` writes the engine input.
+        ``sample_weight`` (float [B]) goes to the row weights the head reads in the ``"sample"`` weighting mode."""
         if x_u8.dim() == 4 and tuple(x_u8.shape[1:3]) != (self.image_size, self.image_size):
             if x_u8.shape[0] != self.batch or x_u8.shape[3] != 3 or x_u8.dtype != torch.uint8:
                 raise ValueError(f"set_input: expected uint8 [{self.batch}, H, W, 3], got {tuple(x_u8.shape)} {x_u8.dtype}")
@@ -983,11 +1038,21 @@ class ResNet50Engine:
             self.x_u8.copy_(x_u8.view(self.x_u8.shape), non_blocking=True)
         if labels is not None:
             self.labels.copy_(labels, non_blocking=True)
+        if sample_weight is not None:
+            _set_row_weight(self, sample_weight)
 
     def set_augment_step(self, t: int) -> None:
         """Step word the next training forward's augmentation reads (the optimizer's step counter)."""
         if self._augmenter is not None:
             self._augmenter.set_step(t)
+
+    def set_weighting(self, mode: Optional[str], training: bool = True) -> bool:
+        """Per-row loss weights of the training or evaluation head (see the module-level `set_weighting`)."""
+        return set_weighting(self, mode, training)
+
+    def set_class_weight(self, table: torch.Tensor) -> None:
+        """New values of the class-weight table (float [K]); no graph needs capturing again."""
+        set_class_weight(self, table)
 
     def set_distillation(self, distillation) -> None:
         """Distil from ``distillation.teacher`` (a `train.losses.Distillation`; None: plain training) in the training
@@ -1175,8 +1240,14 @@ class EngineTrainStep:
     def _opt_state(self):
         return self._opt().state
 
-    def load(self, x_u8: torch.Tensor, labels: torch.Tensor) -> None:
-        self.engine.set_input(x_u8, labels)
+    def load(self, x_u8: torch.Tensor, labels: torch.Tensor, sample_weight: Optional[torch.Tensor] = None) -> None:
+        self.engine.set_input(x_u8, labels, sample_weight)
+
+    def drop_graphs(self) -> None:
+        """Forget the captured graphs (the engine's weighting mode changed): the next `run` captures them again."""
+        if self.use_graph and self._captured:
+            self.graph = self.accum_graph = None
+            self._captured = False
 
     def run(self) -> None:
         if not self._captured:
@@ -1237,6 +1308,10 @@ class EngineEvalStep:
             self.graph.replay()
         else:
             self.engine.forward(training=False)
+
+    def drop_graphs(self) -> None:
+        """Forget the captured graph (the engine's weighting mode changed): the next `run` captures it again."""
+        self.graph = None
 
     def result(self) -> Tuple[float, float]:
         self._host_stats.copy_(self.engine.stats, non_blocking=True)

@@ -56,7 +56,10 @@ def install(trainer_module, enabled: bool, log_models: bool) -> None:
         return
 
     def fit(self, x, steps_per_epoch=None, epochs=1, *args, **kw):
-        cb = _AutologCallback(log_models, {"epochs": epochs, "steps_per_epoch": steps_per_epoch})
+        params = {"epochs": epochs, "steps_per_epoch": steps_per_epoch}
+        if kw.get("class_weight") is not None:   # as Keras's autolog records fit's class_weight
+            params["class_weight"] = kw["class_weight"]
+        cb = _AutologCallback(log_models, params)
         cbs = list(kw.pop("callbacks", None) or []) + [cb]
         return _orig_fit(self, x, steps_per_epoch, epochs, *args, callbacks=cbs, **kw)
 

@@ -7,10 +7,15 @@ P1/03:204-234,325-358, P2/03:206) on top of two execution backends:
   autograd computes gradients into the same kind of flat buffer (`FlatParams`), so optimizers, callbacks and the
   distributed wrapper are shared.
 
-Datasets are iterables of ``(images uint8 [B,H,W,3], labels int64 [B])`` (see `loader.Converter.make_dataset`).
+Datasets are iterables of ``(images uint8 [B,H,W,3], labels int64 [B])`` (see `loader.Converter.make_dataset`), or of
+``(images, labels, sample_weight float [B])``.  Keras 3's loss weighting: ``fit(class_weight={class: weight})`` or
+per-row sample weights scale each row's loss, and the batch loss is ``(1/B) sum_n w_n l_n`` (``sum_over_batch_size``, not
+divided by the sum of the weights); accuracy is not weighted.
 """
 from __future__ import annotations
 
+import math
+import numbers
 import time
 from collections import deque
 from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple
@@ -25,6 +30,46 @@ from ..parallel import core as dist_core
 
 def _is_engine(model) -> bool:
     return hasattr(model, "param_specs") and hasattr(model, "forward") and hasattr(model, "bind_grad_buffer")
+
+
+def _num_classes(model) -> Optional[int]:
+    """Classes of a native engine or a torch module (``num_classes``, else its last Linear layer's outputs)."""
+    k = getattr(model, "num_classes", None)
+    if k is None and isinstance(model, torch.nn.Module):
+        lin = [m for m in model.modules() if isinstance(m, torch.nn.Linear)]
+        k = lin[-1].out_features if lin else None
+    return None if k is None else int(k)
+
+
+def class_weight_table(class_weight: Dict[int, float], num_classes: Optional[int]) -> torch.Tensor:
+    """Keras ``class_weight`` -> float32 [K] table: ``class_weight.get(c, 1.0)`` for every class c.  Keys must be ints in
+    [0, K), values finite floats >= 0; anything else raises ValueError."""
+    if not isinstance(class_weight, dict):
+        raise ValueError(f"class_weight must be a dict {{class index: weight}}, got {type(class_weight).__name__}")
+    if num_classes is None:
+        raise ValueError("class_weight: the model's number of classes is unknown (no num_classes, no Linear layer)")
+    table = torch.ones(num_classes, dtype=torch.float32)
+    for c, w in class_weight.items():
+        if isinstance(c, bool) or not isinstance(c, numbers.Integral) or not 0 <= int(c) < num_classes:
+            raise ValueError(f"class_weight: key {c!r} is not a class index in [0, {num_classes})")
+        if isinstance(w, bool) or not isinstance(w, numbers.Real) or not math.isfinite(float(w)) or float(w) < 0:
+            raise ValueError(f"class_weight[{c}] = {w!r}: weights must be finite numbers >= 0")
+        table[int(c)] = float(w)
+    return table
+
+
+def _unpack(batch, what: str):
+    """(x, y, sample_weight or None) of an ``(x, y)`` or ``(x, y, sample_weight)`` batch."""
+    if not isinstance(batch, (tuple, list)) or len(batch) not in (2, 3):
+        raise ValueError(f"{what}: batches must be (x, y) or (x, y, sample_weight) tuples")
+    w = batch[2] if len(batch) == 3 else None
+    if w is not None:
+        w = torch.as_tensor(w)
+        if not w.is_floating_point() or w.dim() != 1 or w.shape[0] != len(batch[1]):
+            raise ValueError(f"{what}: sample_weight must be a float tensor [B] with one weight per row, got "
+                             f"{w.dtype} {tuple(w.shape)}")
+        w = w.float()
+    return batch[0], batch[1], w
 
 
 class _EngineBackend:
@@ -50,6 +95,22 @@ class _EngineBackend:
         # when distilling: training steps also report the student and distillation terms.
         self._slot = _stats_len(engine)
         self._free = [torch.zeros(self._slot, dtype=torch.float32).pin_memory() for _ in range(4)]
+        self._class_weighted = False
+
+    def set_class_weight(self, table: Optional[torch.Tensor]) -> None:
+        """Weight the training loss by class (float [K] table; None: no class weights) from the next batch on."""
+        self._class_weighted = table is not None
+        if table is not None:
+            self.engine.set_class_weight(table)   # an async copy: captured graphs read the same table
+
+    def _weighting(self, training: bool, w) -> None:
+        """The head's weighting mode for this batch; when it changes, the captured graphs (which launched the other
+        head kernel) are dropped and captured again on their next run."""
+        mode = "sample" if w is not None else ("class" if training and self._class_weighted else None)
+        if self.engine.set_weighting(mode, training):
+            for step in (self._step, self._eval_step):
+                if step is not None:
+                    step.drop_graphs()
 
     @property
     def step(self):
@@ -87,14 +148,16 @@ class _EngineBackend:
             self._free.append(buf)
         return out
 
-    def train_batch(self, x, y) -> None:
-        self.step.load(x, y)
+    def train_batch(self, x, y, w=None) -> None:
+        self._weighting(True, w)
+        self.step.load(x, y, w)
         self.step.run()
         self._enqueue_result(self._slot)
 
-    def eval_batch(self, x, y) -> None:
+    def eval_batch(self, x, y, w=None) -> None:
         step = self.eval_step  # (builds the engine on first use)
-        self.engine.set_input(x, y)
+        self._weighting(False, w)
+        self.engine.set_input(x, y, w)
         step.run()
         self._enqueue_result()
 
@@ -191,6 +254,21 @@ class _ModuleBackend:
             optimizer.attach(self.flat.params, self.flat.grads, None, segments=self.flat.ranges)
         self._results: deque = deque()
         self.batch = None
+        self._class_weight: Optional[torch.Tensor] = None
+
+    def set_class_weight(self, table: Optional[torch.Tensor]) -> None:
+        self._class_weight = None if table is None else table.to(self.device)
+
+    def _row_weights(self, y, mix, w):
+        """Per-row loss weights (None: unweighted): the batch's sample weights, else the class table at each row's
+        target class (the heavier label of a MixUp / CutMix row), as the engines' weighted heads read them."""
+        from ..models.augment import target_argmax
+
+        if w is not None:
+            return w.to(self.device, non_blocking=True)
+        if self._class_weight is not None:
+            return self._class_weight[target_argmax(y, mix)]
+        return None
 
     def _prep(self, x) -> torch.Tensor:
         x = torch.as_tensor(x).to(self.device, non_blocking=True)
@@ -209,7 +287,7 @@ class _ModuleBackend:
         key = augment_key(getattr(self.module, "augmentation_seed", 0), dist_core.rank())
         return augment_batch_reference(self.module.augmentation, x.to(self.device, non_blocking=True), key, opt.t)
 
-    def train_batch(self, x, y) -> None:
+    def train_batch(self, x, y, w=None) -> None:
         from ..models.augment import distillation_reference, soft_targets, target_argmax
 
         self.module.train()
@@ -228,30 +306,38 @@ class _ModuleBackend:
                 t_logits = d.teacher(self._prep(x)).float()
         logits = self.module(self._prep(x)).float()
         eps = self.label_smoothing
+        rw = self._row_weights(y, mix, w)
         if d is not None:
             rows = distillation_reference(logits, t_logits, y, mix, eps, d.alpha, d.temperature)
-            loss, ce, kd = (r.mean() for r in rows)
+            loss, ce, kd = (r.mean() if rw is None else (r * rw).mean() for r in rows)
             acc = (logits.argmax(1) == target_argmax(y, mix)).float().mean()
             loss.backward()
             self.optimizer.step()
             self._results.append(torch.stack([loss.detach(), acc, ce.detach(), kd.detach()]))
             return
+        target = y if mix is None and eps == 0 else soft_targets(y, logits.shape[1], mix, eps)
+        if rw is not None:   # (1/B) sum_n w_n l_n
+            loss = (torch.nn.functional.cross_entropy(logits, target, reduction="none") * rw).mean()
+        else:
+            loss = torch.nn.functional.cross_entropy(logits, target)
         if mix is None and eps == 0:
-            loss = torch.nn.functional.cross_entropy(logits, y)
             acc = (logits.argmax(1) == y).float().mean()
         else:
-            loss = torch.nn.functional.cross_entropy(logits, soft_targets(y, logits.shape[1], mix, eps))
             acc = (logits.argmax(1) == target_argmax(y, mix)).float().mean()
         loss.backward()
         self.optimizer.step()
         self._results.append(torch.stack([loss.detach(), acc.detach()]))
 
     @torch.no_grad()
-    def eval_batch(self, x, y) -> None:
+    def eval_batch(self, x, y, w=None) -> None:
         self.module.eval()
         y = torch.as_tensor(y).to(self.device, non_blocking=True)
         logits = self.module(self._prep(x)).float()
-        loss = torch.nn.functional.cross_entropy(logits, y, label_smoothing=self.label_smoothing)
+        if w is not None:   # evaluation weights only the batch's own sample weights, never class_weight
+            loss = (torch.nn.functional.cross_entropy(logits, y, label_smoothing=self.label_smoothing,
+                                                      reduction="none") * w.to(self.device)).mean()
+        else:
+            loss = torch.nn.functional.cross_entropy(logits, y, label_smoothing=self.label_smoothing)
         acc = (logits.argmax(1) == y).float().mean()
         self._results.append(torch.stack([loss, acc]))
 
@@ -298,6 +384,7 @@ class Trainer:
         self.optimizer = None
         self.backend = None
         self.distillation = None   # the compiled `losses.Distillation`, if any
+        self.class_weight: Optional[Dict[int, float]] = None   # of the last fit()
         self.metrics_names = ["loss"]
         self.stop_training = False
         self.steps_per_epoch: Optional[int] = None
@@ -338,9 +425,19 @@ class Trainer:
     # ------------------------------------------------------------------------------------------------ fit
     def fit(self, x: Iterable, steps_per_epoch: Optional[int] = None, epochs: int = 1, verbose: int = 1,
             validation_data: Optional[Iterable] = None, validation_steps: Optional[int] = None,
-            callbacks: Optional[List[Callback]] = None, initial_epoch: int = 0, **_ignored) -> History:
+            callbacks: Optional[List[Callback]] = None, initial_epoch: int = 0,
+            class_weight: Optional[Dict[int, float]] = None, sample_weight=None, **_ignored) -> History:
+        """``class_weight`` ({class index: weight}, Keras 3): each training row's loss is weighted by its class's weight
+        (1.0 for a class not in the dict); for a MixUp / CutMix row the class is the heavier label of its mixed target.
+        Sample weights come with the batches, ``(x, y, sample_weight)``; the two cannot be combined."""
         if self.backend is None:
             raise RuntimeError("call compile() before fit()")
+        if sample_weight is not None:
+            raise ValueError("fit(sample_weight=...) is not supported when x is a dataset: yield (x, y, sample_weight) "
+                             "batches instead")
+        table = None if class_weight is None else class_weight_table(class_weight, _num_classes(self.model))
+        self.class_weight = class_weight
+        self.backend.set_class_weight(table)
         if steps_per_epoch is None:
             steps_per_epoch = len(x)  # finite datasets only
         self.steps_per_epoch = steps_per_epoch
@@ -359,14 +456,18 @@ class Trainer:
             for b in range(steps_per_epoch):
                 cbs.call("on_train_batch_begin", b, {})
                 try:
-                    xb, yb = next(it)
+                    batch = next(it)
                 except StopIteration:
                     it = iter(x)
                     try:
-                        xb, yb = next(it)
+                        batch = next(it)
                     except StopIteration:
                         raise ValueError("fit(): the dataset yields no batches (fewer rows than batch_size?)") from None
-                self.backend.train_batch(xb, yb)
+                xb, yb, wb = _unpack(batch, "fit()")
+                if wb is not None and table is not None:
+                    raise ValueError("fit(): cannot use class_weight and sample_weight at the same time: the dataset "
+                                     "yields (x, y, sample_weight) batches")
+                self.backend.train_batch(xb, yb, wb)
                 steps_run += 1
                 for r in self.backend.pop_results(keep=1):  # lag one step: keeps H2D/compute overlapped
                     for i, v in enumerate(r):
@@ -425,16 +526,16 @@ class Trainer:
         k = 0
         while steps is None or k < steps:
             try:
-                xb, yb = next(it)
+                batch = next(it)
             except StopIteration:
                 if steps is None:
                     break
                 it = iter(x)
                 try:
-                    xb, yb = next(it)
+                    batch = next(it)
                 except StopIteration:
                     break  # empty dataset
-            self.backend.eval_batch(xb, yb)
+            self.backend.eval_batch(*_unpack(batch, "evaluate()"))
             k += 1
             for l, a in self.backend.pop_results(keep=2):  # bounded queue; lag keeps H2D / compute overlapped
                 tot_loss += l
